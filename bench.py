@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- committed slots/sec of the quorum-vote hot path on B200.
+"""bench.py -- committed slots/sec of the quorum-vote hot path on H100.
 
 Workload (BASELINE.json configs[1], "cfg2"): MultiPaxos, 5 acceptors (f=2),
 thrifty quorum of 3, 2^20 slots in flight per GPU per step.  One STEP is one
@@ -16,8 +16,14 @@ buffers per step, > L2 in total, fresh state region per step);
 fpx_step_wait) from pinned host buffers: H2D of the Phase2a and Phase2b batches,
 D2H of the Phase2b and Chosen replies, double-buffered.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
   python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned to its caller (rank 0):
+phase2b.npy (a fixed seeded sample of 2^19 of the Phase2b records), chosen.npy (every Chosen record),
+watermark.npy and counts.npy (Phase2b, Nack and Chosen records returned; the workload sends no stale Phase2a,
+so there are no Nack records to write), all float64 (exact for int32).  The inputs depend only on the
+arguments, so two builds can be compared output for output.
 """
 import argparse
 import ctypes
@@ -65,26 +71,26 @@ def parse():
     ap.add_argument("--cpu-sample-slots", type=int, default=SLOTS_PER_STEP)
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the extra keys (cfg5 on the same GPUs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     return ap.parse_args()
 
 
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel`, from the
-    committed ncu --set full capture (profiles/r2b_traffic.json); None if absent."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r2b_traffic.json")) as f:
-            k = json.load(f)[kernel]
-        return int(k["dram_bytes_read"] + k["dram_bytes_write"])
-    except Exception:
-        return None
-
-
 def peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 (not measured)"
+
+
+DUMP_P2B_ROWS = 1 << 19   # sampled Phase2b records: 16 MB as float64 next to the 16 MB of Chosen records
+
+
+def dump_outputs(dirname, p2b, n_p2b, n_nack, chosen, n_chosen, wm):
+    """The last timed step's replies (device tensors, valid prefixes n_*) as float64 .npy files."""
+    os.makedirs(dirname, exist_ok=True)
+    p2b = p2b[:n_p2b].cpu().numpy()
+    rows = np.sort(np.random.default_rng(0).choice(n_p2b, size=min(n_p2b, DUMP_P2B_ROWS), replace=False))
+    out = {"phase2b": p2b[rows], "chosen": chosen[:n_chosen].cpu().numpy(), "watermark": wm.cpu().numpy(),
+           "counts": np.array([n_p2b, n_nack, n_chosen])}
+    for name, a in out.items():
+        np.save(os.path.join(dirname, name + ".npy"), a.astype(np.float64))
 
 
 # --------------------------------------------------------------------------- CPU arms (oracle port)
@@ -266,7 +272,7 @@ def main():
     K, W = args.steps, max(args.warmup, 3)
     S = K + W
     KI = min(K, 20)          # instrumented steps (CUDA events around every kernel): per-kernel durations
-    KE = min(K, 10)          # e2e steps: PCIe-bound and ~12x longer each, a bounded sample keeps the run short
+    KE = min(K, 10)          # e2e steps: PCIe-bound and ~8x longer each, a bounded sample keeps the run short
     SE = KE + W
     total_windows = S + KI + (0 if args.no_e2e else SE)
     if total_windows * SLOTS_PER_STEP * N >= (1 << 31):
@@ -343,6 +349,8 @@ def main():
     assert r.status == 0 and r.n_chosen == SLOTS_PER_STEP and r.n_nack == 0
     exp_wm = (S * SLOTS_PER_STEP) * N + rank
     assert r.watermark == exp_wm, (r.watermark, exp_wm)
+    if args.dump_outputs and rank == 0:   # before the instrumented pass reuses the output buffers
+        dump_outputs(args.dump_outputs, d_out_p2b, r.n_p2b, r.n_nack, d_out_chosen, r.n_chosen, d_wm)
     global_prefix = None
     if N > 1:   # every shard's frontier after step S, as the peers stored it into THIS rank's table
         global_prefix, fr = eng.global_watermark(epoch=S)
@@ -355,7 +363,7 @@ def main():
     ms_max = float(t.item())
     value = N * K * SLOTS_PER_STEP / (ms_max * 1e-3)
 
-    # ---- per-kernel durations: a second, instrumented pass (CUDA events between the kernels cost ~5 us
+    # ---- per-kernel durations: a second, instrumented pass (CUDA events between the kernels cost several us
     # each on the stream, so they stay out of the pass that produces `value`)
     e_i0, e_i1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e_i0.record(ext)
@@ -449,11 +457,9 @@ def main():
         step_ms = ms_max / K
         dominant = "tally_kernel" if tally_ms >= acc_ms else "acceptor_phase2a_kernel"
         kern = {"acceptor_phase2a_kernel": {"ms": acc_ms, "GB/s": acc_gbs, "frac": acc_gbs / peak,
-                                            "algorithmic_bytes_per_launch": B_ACCEPTOR * SLOTS_PER_STEP,
-                                            "traffic": ncu_traffic("acceptor_phase2a_kernel")},
+                                            "algorithmic_bytes_per_launch": B_ACCEPTOR * SLOTS_PER_STEP},
                 "tally_kernel": {"ms": tally_ms, "GB/s": tally_gbs, "frac": tally_gbs / peak,
                                  "algorithmic_bytes_per_launch": B_TALLY_FUSED * SLOTS_PER_STEP,
-                                 "traffic": ncu_traffic("tally_kernel"),
                                  "note": "ProxyLeader.handlePhase2b + the co-located replica's handleChosen and the "
                                          "first-hole scan in one launch: 16Q+24 (tally) + 8 (log put) + 8 (scan) B/slot"},
                 "arm_kernel": {"ms": arm_ms}}
@@ -465,11 +471,11 @@ def main():
             "config": config_dict(N),
             # the dominant kernel by time of the step (CUDA events of the instrumented pass)
             "roofline": {"bound": "hbm", "kernel": dominant, "achieved": kern[dominant]["GB/s"], "peak": peak,
-                         "unit": "GB/s", "frac": kern[dominant]["frac"], "traffic": kern[dominant]["traffic"],
+                         "unit": "GB/s", "frac": kern[dominant]["frac"],
                          "algorithmic_bytes_per_launch": kern[dominant]["algorithmic_bytes_per_launch"],
                          "ms_per_launch": kern[dominant]["ms"], "peak_source": peak_src,
                          "timing": f"CUDA events on the engine's stream around every kernel of {KI} instrumented steps "
-                                   "run right after the timed region (events between kernels cost ~5 us each, so the "
+                                   "run right after the timed region (events between kernels cost several us each, so the "
                                    "pass that produces `value` carries none)"},
             "kernels": dict(kern, **{"whole_step_GB/s": B_SLOT * SLOTS_PER_STEP / (step_ms * 1e-3) / 1e9,
                                      "whole_step_frac": B_SLOT * SLOTS_PER_STEP / (step_ms * 1e-3) / 1e9 / peak}),

@@ -1,6 +1,6 @@
-"""frankenpaxos_b200 -- B200-native engine for FrankenPaxos's quorum-vote hot path.
+"""frankenpaxos_b200 -- H100-native engine for FrankenPaxos's quorum-vote hot path.
 
-The product is libfpx.so (CUDA, sm_100a) behind the C ABI of include/fpx.h; this
+The product is libfpx.so (CUDA, sm_90a) behind the C ABI of include/fpx.h; this
 package is the Python handle over it plus mirrors of the reference's classes on
 the path (quorums.Grid / SimpleMajority, multipaxos.Config / ProxyLeader /
 Acceptor).  Importing the package does not need a GPU; constructing an Engine

@@ -1,4 +1,4 @@
-"""In-tree build of libfpx.so (sm_100a only).  `python -m frankenpaxos_b200.build`."""
+"""In-tree build of libfpx.so (sm_90a only).  `python -m frankenpaxos_b200.build`."""
 import os
 import subprocess
 import sys
@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libfpx.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-Wall,-Wextra,-Wno-unused-parameter",
     "-shared", "-cudart", "static",

@@ -1,8 +1,8 @@
-// fpx_common.cuh -- shared layouts and device helpers of the sm_100a kernels.
+// fpx_common.cuh -- shared layouts and device helpers of the sm_90a kernels.
 //
 // Everything here is integer scatter/gather + order-preserving prefix logic
 // bounded by HBM/L2 bandwidth; there is no GEMM-shaped work, hence no
-// tcgen05/TMEM.  What matters (DESIGN.md "kernels"): one 128-bit load per
+// wgmma.  What matters (DESIGN.md "kernels"): one 128-bit load per
 // message record, fully coalesced warp chunks, at most one 32-byte sector per
 // random state access (a proxy-leader row IS one sector for <= 6 voters),
 // warp ballots/shuffles/redux for the in-order logic, and PERSISTENT
@@ -35,7 +35,8 @@ constexpr int kThreads = 256;                     // threads per CTA of the rang
 constexpr int kWarps = kThreads / 32;
 constexpr int kMaxKeys = FPX_MAX_ACCEPTORS;       // acceptors tracked by the round scan (lane = key)
 constexpr int kMaxConflicts = 1024;
-constexpr int kMaxGrid = 148 * 8;                 // upper bound on CTAs of a cooperative launch
+constexpr int kSms = 132;                         // H100 SXM; sizes grid-stride launches that need no exact count
+constexpr int kMaxGrid = kSms * 8;                // upper bound on CTAs of a cooperative launch
 constexpr uint32_t kTsBadVoter = 1u, kTsAnomaly = 2u, kTsPoison = 4u, kTsVanillaRound = 8u;  // DevStatus::ts_flags
 
 // Device-resident status block (one per engine).

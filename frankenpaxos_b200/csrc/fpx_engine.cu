@@ -1,6 +1,6 @@
 // fpx_engine.cu -- host side of libfpx.so: the C ABI of include/fpx.h.
 //
-// One fpx_engine owns, on one B200: the vote cells of every acceptor of the
+// One fpx_engine owns, on one GPU: the vote cells of every acceptor of the
 // config (flat slot x voter array of 64-bit {round, value} cells), the proxy
 // leader's per-(slot, round) rows, the overflow table for secondary rounds, the
 // replica log, one CUDA stream, and pinned/device staging for the host-pointer
@@ -414,7 +414,7 @@ int fpx_retire_below(fpx_engine* e, int32_t slot) {
   if (new_base < g.base_local) new_base = g.base_local;
   const int count = (int)std::min<long long>(new_base - g.base_local, g.local_slots);
   if (count == 0) return FPX_OK;
-  recycle_kernel<<<std::min(count * 8 + 255, 148 * 2048) / 256 + 1, 256, 0, e->stream>>>(g, e->rows, e->votes, e->rlog, 0, count);
+  recycle_kernel<<<std::min(count * 8 + 255, kSms * 2048) / 256 + 1, 256, 0, e->stream>>>(g, e->rows, e->votes, e->rlog, 0, count);
   e->launches++;
   CK(e, cudaGetLastError());
   g.base_local = (int32_t)new_base;
@@ -674,7 +674,8 @@ int fpx_step_dev(fpx_engine* e, const fpx_p2a* d_arm, int32_t n_arm, const fpx_p
   // The arm batch and the acceptor batch touch disjoint state (proxy-leader rows / vote cells), so their
   // order is free; the acceptors go first so that the rows armed last are still L2-resident when the
   // votes are tallied.  The co-located replica (handleChosen + watermark) rides in the tally kernel.
-  // (Running the arm batch inside the acceptor kernel was tried and lost: profiles/experiments.md.)
+  // (Running the arm batch inside the acceptor kernel was tried and lost: the rows were cold again
+  // for the tally and the acceptor's second pass slowed down.)
   if (ev) CK(e, cudaEventRecord(ev[0], e->stream));
   int c = fpx_acceptor_phase2a_dev(e, d_p2a, n_p2a, d_out_p2b, d_out_nack);
   if (c != FPX_OK) return c;

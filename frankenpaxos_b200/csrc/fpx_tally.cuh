@@ -22,7 +22,7 @@
 //              row load; per-batch statistics (slot window, rounds) on the side
 //     barrier
 //     phase B  SWEEP (steady state): the window's rows are read once, coalesced
-//              (one 256-bit load per row, every CTA a contiguous run of rows),
+//              (one 32-byte sector per 8 row words, every CTA a contiguous run of rows),
 //              c(key) evaluated per row; a key completed by vote i of this batch sets
 //              bit i of a bitmap and keeps {i, value} in the CTA's shared memory;
 //           or EXACT (fallback): one divergent row load per vote and the reference's
@@ -90,19 +90,19 @@ constexpr int kTallyUnroll = FPX_TALLY_UNROLL;   // chunks of 32 votes per warp 
 constexpr int kChunkVotes = 1024; // votes per rank chunk (one bitmap word per lane)
 constexpr uint32_t kNoVote = 0xffffffffu;
 // One CTA of 32 warps per SM: several CTAs per SM spread up to 2x in duration (their loads queue behind
-// each other in the SM's L1TEX, B300_MICROARCH "Multi-CTA spread"), and every phase ends at a grid barrier.
+// each other in the SM's L1TEX), and every phase ends at a grid barrier.
 constexpr int kTT = FPX_TT;
 constexpr int kTW = kTT / 32;
 
-// One proxy-leader row from L2 with a single 256-bit load per 8 words (LDG.E.256, sm_100+).
+// One proxy-leader row from L2, two 128-bit loads per 8 words (one 32-byte sector; sm_90 has no
+// 256-bit load).  Both halves are issued before either is used.
 template <int ROWW>
 __device__ __forceinline__ void load_row(const uint32_t* p, uint32_t (&w)[ROWW]) {
 #pragma unroll
-  for (int q = 0; q < ROWW / 8; ++q) {
-    asm volatile("ld.global.cg.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(w[8 * q]), "=r"(w[8 * q + 1]), "=r"(w[8 * q + 2]), "=r"(w[8 * q + 3]),
-                   "=r"(w[8 * q + 4]), "=r"(w[8 * q + 5]), "=r"(w[8 * q + 6]), "=r"(w[8 * q + 7])
-                 : "l"(p + 8 * q));
+  for (int q = 0; q < ROWW / 4; ++q) {
+    asm volatile("ld.global.cg.v4.b32 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(w[4 * q]), "=r"(w[4 * q + 1]), "=r"(w[4 * q + 2]), "=r"(w[4 * q + 3])
+                 : "l"(p + 4 * q));
   }
 }
 
@@ -184,7 +184,7 @@ __device__ __forceinline__ uint32_t vote_rank(const TallyParams& P, const uint32
 template <int ROWW, bool kEmit>
 __device__ __forceinline__ void tally_sweep(const TallyParams& P, int w_lo, int w_hi, int R, int rows_per_cta, bool keep,
                                             uint2* s_keep, const uint32_t* s_ccx, uint32_t out_base, int& mx) {
-  constexpr int U = ROWW == 8 ? 4 : (ROWW == 16 ? 2 : 1);
+  constexpr int U = ROWW == 8 ? 2 : 1;   // rows in flight per thread: more spills registers under the 64-register cap
   const Geometry& g = P.g;
   const long long nrows = (long long)w_hi - w_lo + 1;
   const long long r_begin = (long long)blockIdx.x * rows_per_cta;

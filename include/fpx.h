@@ -1,5 +1,5 @@
 /*
- * fpx.h -- C ABI of the B200 quorum-vote engine (libfpx.so).
+ * fpx.h -- C ABI of the H100 quorum-vote engine (libfpx.so).
  *
  * This is the drop-in boundary for the FrankenPaxos quorum-vote hot path.  The
  * reference (mwhittaker/frankenpaxos, Scala) has no FFI; its extension surface

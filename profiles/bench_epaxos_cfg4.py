@@ -10,6 +10,7 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from bench import peaks  # noqa: E402
 from frankenpaxos_b200 import traces as T  # noqa: E402
 from frankenpaxos_b200.epaxos import EpaxosReplica  # noqa: E402
 
@@ -43,17 +44,13 @@ def run(N=1 << 20, f=2, reps=3):
     # algorithmic bytes per message: input row + reply row + cmdLog row read+write (+ leader row for lead / responses)
     alg = {"lead": 4 * (8 + n) + 64 + 512, "preaccept": 4 * (6 + 2 * n) + 4 * (4 + n) + 2 * 64,
            "preacceptok": 4 * (6 + n) + 4 * (2 + n) + 4 * 10 + 64}
-    peak = 6488.7
-    try:
-        peak = float(json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["hbm_gbs"])
-    except Exception:
-        pass
+    peak, _ = peaks()
     return {"config": "cfg4: EPaxos n=5 f=2, 2^20 instances, BernoulliSingleKeyWorkload(0.2), replica 0's view, device-resident rows",
             "fast_commits": ev_counts[0], "slow_paths": ev_counts[1],
             "calls": {k: {"messages": msgs[k], "kernel_ms": best[k], "messages_per_s": msgs[k] / (best[k] * 1e-3),
                           "algorithmic_bytes_per_message": alg[k],
                           "GB/s": alg[k] * msgs[k] / (best[k] * 1e-3) / 1e9,
-                          "frac_of_measured_hbm_peak": alg[k] * msgs[k] / (best[k] * 1e-3) / 1e9 / peak} for k in best}}
+                          "frac_of_hbm_peak": alg[k] * msgs[k] / (best[k] * 1e-3) / 1e9 / peak} for k in best}}
 
 
 if __name__ == "__main__":

@@ -35,7 +35,7 @@ def timed(fn, rounds=10, warm=3):
     ms = []
     for r in range(warm + rounds):
         flush_sink.copy_(flush.view(torch.int32).sum())   # evict L2 between rounds by READING 256 MB: lines stay clean
-                                                            # (a written flush buffer leaves 126 MB of dirty lines whose
+                                                            # (a written flush buffer leaves a whole L2 of dirty lines whose
                                                             # write-back would be billed to the timed kernel)
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

@@ -9,8 +9,8 @@ list of operations + expectations.  tests/test_golden_oracle.py replays them
 against oracle/fpx_oracle.cc; the `-m gpu` tests replay the quorum vectors
 against the CUDA predicates.
 
-Run in the build container only (needs /root/reference):
-    python tests/golden/make_golden.py
+Needs a checkout of the reference; the JSON fixtures are committed, the tests never run this:
+    FPX_REFERENCE=<reference checkout> python tests/golden/make_golden.py
 Sources (relative to the reference root), shared/src/test/scala/:
     quorums/GridTest.scala            :11-102
     quorums/SimpleMajorityTest.scala  :11-63
@@ -30,7 +30,7 @@ import os
 import re
 import sys
 
-REF = os.environ.get("FPX_REFERENCE", "/root/reference")
+REF = os.environ.get("FPX_REFERENCE", "")
 T = os.path.join(REF, "shared/src/test/scala")
 OUT = os.path.dirname(os.path.abspath(__file__))
 

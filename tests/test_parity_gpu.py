@@ -1,7 +1,7 @@
 """Parity of the CUDA path (through the C ABI) against the CPU oracle, bit-exact:
 Phase2b / Nack / Chosen streams INCLUDING ORDER, error status + first offending
 index, final acceptor state (round, maxVotedSlot, voteRound[], voteValue[]) and
-replica log / watermark.  Marked gpu: needs a B200."""
+replica log / watermark.  Marked gpu: needs an H100."""
 import json
 import os
 
