@@ -129,6 +129,8 @@ def lib():
     if hasattr(L, "fpx_debug_set_tally_path"):
         L.fpx_debug_set_tally_path.argtypes = [vp, i32]; L.fpx_debug_set_tally_path.restype = i32
         L.fpx_debug_last_tally_path.argtypes = [vp]; L.fpx_debug_last_tally_path.restype = i32
+    if hasattr(L, "fpx_debug_set_acceptor_segments"):
+        L.fpx_debug_set_acceptor_segments.argtypes = [vp, i32]; L.fpx_debug_set_acceptor_segments.restype = i32
     if L.fpx_abi_version() != 1:
         raise ImportError("libfpx.so ABI version mismatch")
     _lib = L

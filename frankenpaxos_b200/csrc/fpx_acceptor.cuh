@@ -7,15 +7,20 @@
 //   (rejected messages are below the running max, so including them is
 //   harmless): an exclusive keyed prefix-max in delivery order.
 //
-//   Persistent cooperative kernel, every warp owns a contiguous range:
+//   Persistent cooperative kernel.  The batch is cut into S contiguous segments
+//   (S = 1 unless the batch is too large for L2, see acceptor_segments); inside a
+//   segment every warp owns a contiguous range:
 //     pass 1  stream the range once, lane k of the warp accumulates the max round
 //             addressed to acceptor k (warp redux; one instruction when the whole
 //             chunk carries one round -- the steady state);
 //     barrier CTA aggregates -> global; every CTA takes the max over the CTAs
-//             before it (+ the acceptors' rounds at batch start) = its carry-in;
+//             before it in the segment, over every earlier segment and the
+//             acceptors' rounds at batch start = its carry-in;
 //     pass 2  stream the range again (now an L2 hit): accept test, vote cell,
 //             Phase2b reply, maxVotedSlot.  Replies are written at index i
 //             (dense = correct whenever the batch produces no Nack);
+//             then pass 1 of the next segment, and its barrier: pass 1 keeps only
+//             ONE segment resident in L2 (S + 1 barriers in all);
 //     barrier if any Nack was produced (leader change): pass 3 rewrites both
 //             reply streams compacted in delivery order from exact prefix counts.
 //   Vote cell: states(slot) = State(round, value) (:205-208) is one 64-bit
@@ -23,6 +28,8 @@
 //   delivery order, so max == last writer, except "same round, different value"
 //   which is flagged and resolved to last-in-order by the last block.
 #pragma once
+#include <algorithm>
+
 #include "fpx_common.cuh"
 
 namespace fpx {
@@ -39,8 +46,9 @@ struct AcceptorParams {
   int32_t* acc_round;              // num_keys
   int32_t* acc_max_voted;          // num_keys
   uint32_t* accept_bits;           // ceil(n/32)
-  int32_t* g_agg;                  // [grid][kMaxKeys] per-CTA max round per acceptor
-  uint32_t* g_wacc;                // [grid*kAW] accepted records per warp range
+  int32_t* g_agg;                  // [2][kMaxGrid][kMaxKeys] per-CTA max round per acceptor (segments alternate)
+  uint32_t* g_wacc;                // [segments][grid*kAW] accepted records per warp range
+  int32_t segments;                // 1 .. kAccMaxSegments
   uint32_t parity;                 // which nack counter this launch uses
   int32_t append;                  // 1: continue the reply streams of the previous launch (chunked host call)
   DevStatus* st;
@@ -54,6 +62,16 @@ constexpr int kAccUnroll = 4;
 #endif
 constexpr int kAT = FPX_AT;
 constexpr int kAW = kAT / 32;
+constexpr int kAccMaxSegments = 8;
+// Segments of a batch of n records: pass 1 pins at most half of the L2 (16 B per record), the other half
+// takes pass 2's replies and vote cells.  More segments cost a grid barrier each and shorten every warp's
+// run: cfg2 (3 * 2^20 records) on H100's 50 MB L2 takes 2; 4 measured 11 us slower (DESIGN.md section 4).
+inline int acceptor_segments(long long n, long long l2_bytes) {
+  const long long seg_bytes = l2_bytes / 2;
+  if (seg_bytes <= 0) return 1;
+  const long long s = (n * 16 + seg_bytes - 1) / seg_bytes;
+  return (int)std::max(1ll, std::min((long long)kAccMaxSegments, s));
+}
 __device__ __forceinline__ int grp_of(int dst) { return dst >> 16; }
 
 // decode + validate one Phase2a record; key = global acceptor id or -1
@@ -90,7 +108,8 @@ __device__ __forceinline__ void acceptor_apply(const AcceptorParams& P, int4* ou
   const Geometry& g = P.g;
   const unsigned full = 0xffffffffu;
   // the reply stream is write-once: evict_first gets it written back while this kernel
-  // still runs instead of during the next kernel's reads
+  // still runs instead of during the next kernel's reads.  This is also the last read of
+  // the records pass 1 pinned (evict_last): the evict_first load releases them.
   const unsigned long long pol_out = l2_policy_evict_first();
   for (int base = wlo; base < whi; base += 32 * kAccUnroll) {
     int4 rec[kAccUnroll];
@@ -98,7 +117,7 @@ __device__ __forceinline__ void acceptor_apply(const AcceptorParams& P, int4* ou
 #pragma unroll
     for (int u = 0; u < kAccUnroll; ++u) {
       int i = base + u * 32 + lane;
-      rec[u] = (i < whi) ? ld_cg(P.in + i) : make_int4(0, -1, 0, -1);
+      rec[u] = (i < whi) ? ld_hint(P.in + i, pol_out) : make_int4(0, -1, 0, -1);
       cell[u] = 0; old[u] = 0;
     }
 #pragma unroll
@@ -187,35 +206,13 @@ __device__ __forceinline__ void acceptor_apply(const AcceptorParams& P, int4* ou
   }
 }
 
-__global__ void __launch_bounds__(kAT, 1024 / kAT) acceptor_phase2a_kernel(AcceptorParams P) {
+// Pass 1 over [wlo, whi): lane k returns the max round addressed to acceptor k.  The records are
+// tagged evict_last in L2 so that pass 2 (which also writes 24 B/record of replies and vote cells
+// through L2) still finds them there; acceptor_segments bounds how much of the batch that pins, and
+// pass 2's evict_first load releases them.
+__device__ __forceinline__ int acceptor_scan(const AcceptorParams& P, int wlo, int whi, int lane) {
   const Geometry& g = P.g;
-  extern __shared__ int s_mv[];  // [num_keys][kAT] private maxVotedSlot columns
-  __shared__ int s_wagg[kAW][kMaxKeys];
-  __shared__ int s_tmp[kAW][kMaxKeys];
-  __shared__ int s_win;
-
   const unsigned full = 0xffffffffu;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int total_warps = gridDim.x * kAW;
-  const int per = (((P.n + total_warps - 1) / total_warps) + 31) & ~31;   // contiguous range of every warp
-  const int gw = blockIdx.x * kAW + warp;
-  const int wlo = (int)min((long long)P.n, (long long)gw * per);
-  const int whi = (int)min((long long)P.n, (long long)wlo + per);
-  uint32_t* nack_ctr = P.parity ? &P.st->nack_total : &P.st->pad[0];
-  uint32_t* nack_other = P.parity ? &P.st->pad[0] : &P.st->nack_total;
-  if (blockIdx.x == 0 && tid == 0) *nack_other = 0;  // the counter the NEXT launch uses
-  // reply-stream bases: 0, or where the previous launch of a chunked call stopped (read by
-  // every CTA before the first grid barrier; rewritten only after the second)
-  const uint32_t base_p2b = P.append ? (uint32_t)__ldcg(&P.st->n_p2b) : 0u;
-  const uint32_t base_nack = P.append ? (uint32_t)__ldcg(&P.st->n_nack) : 0u;
-  int4* const out_p2b = P.out_p2b + base_p2b;
-  int2* const out_nack = P.out_nack + base_nack;
-  for (int k = 0; k < g.num_keys; ++k) s_mv[k * kAT + tid] = INT_MIN;
-  FPX_MARK(P.st->t_acceptor, 0);
-
-  // ---- pass 1: per-acceptor max round of the warp's range (lane = acceptor).
-  // The stream is tagged evict_last in L2 so that pass 2 (which also writes
-  // 88 B/record of replies and vote cells through L2) still finds it there.
   const unsigned long long pol_keep = l2_policy_evict_last();
   int wagg = INT_MIN;
   for (int base = wlo; base < whi; base += 32 * kAccUnroll) {
@@ -250,44 +247,104 @@ __global__ void __launch_bounds__(kAT, 1024 / kAT) acceptor_phase2a_kernel(Accep
       }
     }
   }
-  s_wagg[warp][lane] = wagg;
-  __syncthreads();
-  int cta_agg = INT_MIN;
-  if (warp == 0) {
-#pragma unroll
-    for (int w = 0; w < kAW; ++w) cta_agg = max(cta_agg, s_wagg[w][lane]);
-    __stcg(&P.g_agg[blockIdx.x * kMaxKeys + lane], cta_agg);
-  }
-  FPX_MARK(P.st->t_acceptor, 1);
-  grid_sync(P.st);
-  FPX_MARK(P.st->t_acceptor, 2);
+  return wagg;
+}
 
-  // ---- carry-in: acceptor rounds at batch start + every CTA before this one.
-  // thread t covers CTAs t, t+256, ... for every acceptor: all loads independent.
-  for (int k = 0; k < g.num_keys; ++k) {
-    int v = INT_MIN;
-    for (int c = tid; c < (int)blockIdx.x; c += kAT) v = max(v, __ldcg(&P.g_agg[c * kMaxKeys + k]));
-    v = __reduce_max_sync(full, v);
-    if (lane == 0) s_tmp[warp][k] = v;
-  }
-  __syncthreads();
-  int cta_carry = INT_MIN;
-  if (lane < g.num_keys) {
-    cta_carry = __ldcg(&P.acc_round[lane]);
-#pragma unroll
-    for (int w = 0; w < kAW; ++w) cta_carry = max(cta_carry, s_tmp[w][lane]);
-  }
-  int run = cta_carry;
-  for (int w = 0; w < warp; ++w) run = max(run, s_wagg[w][lane]);
+// Records of warp gw in segment s: a segment is a contiguous run of seg_len records (a multiple of 32
+// when S > 1), inside it warp gw owns [gw*per, (gw+1)*per), so delivery order is (segment, CTA, warp).
+__device__ __forceinline__ void acceptor_range(int n, int seg_len, int per, int s, int gw, int& lo, int& hi) {
+  const long long s_lo = min((long long)n, (long long)s * seg_len), s_hi = min((long long)n, s_lo + seg_len);
+  lo = (int)min(s_hi, s_lo + (long long)gw * per);
+  hi = (int)min(s_hi, (long long)lo + per);
+}
 
-  FPX_MARK(P.st->t_acceptor, 3);
-  // ---- pass 2: decisions + effects, replies at dense positions
-  uint32_t wacc = 0, wnack = 0;
-  acceptor_apply<false>(P, out_p2b, out_nack, wlo, whi, lane, run, 0u, s_mv, wacc, wnack);
-  if (lane == 0) {
-    __stcg(&P.g_wacc[gw], wacc);
-    if (wnack) atomicAdd(nack_ctr, wnack);
+__global__ void __launch_bounds__(kAT, 1024 / kAT) acceptor_phase2a_kernel(AcceptorParams P) {
+  const Geometry& g = P.g;
+  extern __shared__ int s_acc_dyn[];  // [num_keys][kAT] private maxVotedSlot columns, [segments][kAT] carry-ins
+  int* const s_mv = s_acc_dyn;
+  int* const s_run = s_acc_dyn + g.num_keys * kAT;
+  __shared__ int s_wagg[kAW][kMaxKeys];
+  __shared__ int s_tmp[2][kAW][kMaxKeys];
+  __shared__ int s_win;
+
+  const unsigned full = 0xffffffffu;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int total_warps = gridDim.x * kAW;
+  const int S = P.segments;
+  const int seg_len = S == 1 ? P.n : (((P.n + S - 1) / S) + 31) & ~31;
+  const int per = (((seg_len + total_warps - 1) / total_warps) + 31) & ~31;   // contiguous range of every warp
+  const int gw = blockIdx.x * kAW + warp;
+  uint32_t* nack_ctr = P.parity ? &P.st->nack_total : &P.st->pad[0];
+  uint32_t* nack_other = P.parity ? &P.st->pad[0] : &P.st->nack_total;
+  if (blockIdx.x == 0 && tid == 0) *nack_other = 0;  // the counter the NEXT launch uses
+  // reply-stream bases: 0, or where the previous launch of a chunked call stopped (read by
+  // every CTA before the first grid barrier; rewritten only after the last)
+  const uint32_t base_p2b = P.append ? (uint32_t)__ldcg(&P.st->n_p2b) : 0u;
+  const uint32_t base_nack = P.append ? (uint32_t)__ldcg(&P.st->n_nack) : 0u;
+  int4* const out_p2b = P.out_p2b + base_p2b;
+  int2* const out_nack = P.out_nack + base_nack;
+  for (int k = 0; k < g.num_keys; ++k) s_mv[k * kAT + tid] = INT_MIN;
+  FPX_MARK(P.st->t_acceptor, 0);
+
+  // ---- pass 1 of segment 0: per-acceptor max round of the warp's range (lane = acceptor)
+  int wlo, whi;
+  acceptor_range(P.n, seg_len, per, 0, gw, wlo, whi);
+  int wagg = acceptor_scan(P, wlo, whi, lane);
+  // lane k: acceptor k's round before the running segment (batch start, then every earlier segment)
+  int prev = lane < g.num_keys ? __ldcg(&P.acc_round[lane]) : INT_MIN;
+  uint32_t wnack = 0;
+  for (int s = 0; s < S; ++s) {
+    // ---- the CTA's aggregate of segment s -> global (two buffers: segment s-1's is still being read
+    // by CTAs that are not yet past this barrier)
+    if (s > 0) __syncthreads();   // every warp has read s_wagg for segment s-1
+    s_wagg[warp][lane] = wagg;
+    __syncthreads();
+    int32_t* const agg = P.g_agg + (s & 1) * kMaxGrid * kMaxKeys;
+    if (warp == 0) {
+      int cta_agg = INT_MIN;
+#pragma unroll
+      for (int w = 0; w < kAW; ++w) cta_agg = max(cta_agg, s_wagg[w][lane]);
+      __stcg(&agg[blockIdx.x * kMaxKeys + lane], cta_agg);
+    }
+    if (s == 0) FPX_MARK(P.st->t_acceptor, 1);
+    grid_sync(P.st);
+    if (s == 0) FPX_MARK(P.st->t_acceptor, 2);
+
+    // ---- carry-in: rounds before segment s + every CTA before this one in segment s; and the max over
+    // the whole segment, which is part of the next segment's carry.  Thread t covers CTAs t, t+kAT, ...
+    // for every acceptor: all loads independent.
+    for (int k = 0; k < g.num_keys; ++k) {
+      int vb = INT_MIN, va = INT_MIN;
+      for (int c = tid; c < (int)gridDim.x; c += kAT) {
+        const int v = __ldcg(&agg[c * kMaxKeys + k]);
+        va = max(va, v);
+        if (c < (int)blockIdx.x) vb = max(vb, v);
+      }
+      vb = __reduce_max_sync(full, vb);
+      va = __reduce_max_sync(full, va);
+      if (lane == 0) { s_tmp[0][warp][k] = vb; s_tmp[1][warp][k] = va; }
+    }
+    __syncthreads();
+    int run = prev;
+    if (lane < g.num_keys) {
+#pragma unroll
+      for (int w = 0; w < kAW; ++w) { run = max(run, s_tmp[0][w][lane]); prev = max(prev, s_tmp[1][w][lane]); }
+    }
+    for (int w = 0; w < warp; ++w) run = max(run, s_wagg[w][lane]);
+    s_run[s * kAT + tid] = run;   // pass 3 starts from the same carry
+    if (s == 0) FPX_MARK(P.st->t_acceptor, 3);
+
+    // ---- pass 2 of segment s: decisions + effects, replies at dense positions
+    uint32_t wacc = 0;
+    acceptor_apply<false>(P, out_p2b, out_nack, wlo, whi, lane, run, 0u, s_mv, wacc, wnack);
+    if (lane == 0) __stcg(&P.g_wacc[s * total_warps + gw], wacc);
+    // ---- pass 1 of segment s + 1 (published at the top of the next iteration)
+    if (s + 1 < S) {
+      acceptor_range(P.n, seg_len, per, s + 1, gw, wlo, whi);
+      wagg = acceptor_scan(P, wlo, whi, lane);
+    }
   }
+  if (lane == 0 && wnack) atomicAdd(nack_ctr, wnack);
   __syncthreads();
   for (int k = warp; k < g.num_keys; k += kAW) {
     int m = INT_MIN;
@@ -302,25 +359,28 @@ __global__ void __launch_bounds__(kAT, 1024 / kAT) acceptor_phase2a_kernel(Accep
 
   // round after the batch = max over everything (:204); only now is it safe to
   // overwrite the batch-start value every CTA read above
-  if (blockIdx.x == gridDim.x - 1 && warp == 0 && lane < g.num_keys) {
-    int tot = cta_carry;
-#pragma unroll
-    for (int w = 0; w < kAW; ++w) tot = max(tot, s_wagg[w][lane]);
-    P.acc_round[lane] = tot;
-  }
+  if (blockIdx.x == gridDim.x - 1 && warp == 0 && lane < g.num_keys) P.acc_round[lane] = prev;
   const uint32_t total_nacks = __ldcg(nack_ctr);
   if (total_nacks == 0) {
     if (blockIdx.x == 0 && tid == 0) { P.st->n_p2b = (int)base_p2b + P.n; P.st->n_nack = (int)base_nack; }
   } else {
-    // ---- pass 3 (leader change only): exact, compacted reply streams
+    // ---- pass 3 (leader change only): exact, compacted reply streams.  `before` = records accepted
+    // by the warp ranges before this one in delivery order, (segment, warp) major to minor.
     uint32_t before = 0;
-    for (int j = lane; j < gw; j += 32) before += __ldcg(&P.g_wacc[j]);
-    before = __reduce_add_sync(full, before);
-    uint32_t wacc2 = 0, wnack2 = 0;
-    acceptor_apply<true>(P, out_p2b, out_nack, wlo, whi, lane, run, before, s_mv, wacc2, wnack2);
-    if (gw == (int)gridDim.x * kAW - 1 && lane == 0) {
-      P.st->n_p2b = (int)(base_p2b + before + wacc2);
-      P.st->n_nack = (int)base_nack + P.n - (int)(before + wacc2);
+    int j0 = 0;
+    for (int s = 0; s < S; ++s) {
+      const int idx = s * total_warps + gw;
+      uint32_t b = 0;
+      for (int j = j0 + lane; j < idx; j += 32) b += __ldcg(&P.g_wacc[j]);
+      before += __reduce_add_sync(full, b);
+      j0 = idx;
+      acceptor_range(P.n, seg_len, per, s, gw, wlo, whi);
+      uint32_t wacc2 = 0, wnack2 = 0;
+      acceptor_apply<true>(P, out_p2b, out_nack, wlo, whi, lane, s_run[s * kAT + tid], before, s_mv, wacc2, wnack2);
+      if (s == S - 1 && gw == total_warps - 1 && lane == 0) {
+        P.st->n_p2b = (int)(base_p2b + before + wacc2);
+        P.st->n_nack = (int)base_nack + P.n - (int)(before + wacc2);
+      }
     }
   }
 

@@ -168,6 +168,16 @@ __device__ __forceinline__ int4 ld_hint(const int4* p, unsigned long long pol) {
                : "l"(p), "l"(pol));
   return r;
 }
+// 64-bit L2 load tagged evict_last, the policy created in place (it folds into the access's memory
+// descriptor): no 64-bit policy register stays live across a loop that runs at the 64-register cap
+__device__ __forceinline__ unsigned long long ld_u64_evict_last(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("{ .reg .b64 pol; createpolicy.fractional.L2::evict_last.b64 pol, 1.0; "
+               "ld.global.cg.L2::cache_hint.u64 %0, [%1], pol; }"
+               : "=l"(v) : "l"(p));
+  return v;
+}
+
 // Reductions WITHOUT a return value.  atomicMin/atomicMax/atomicOr whose result is unused compile to
 // ATOMG with the destination discarded (RZ), which still holds a scoreboard slot and a return packet;
 // `red` is the fire-and-forget form (REDG).

@@ -69,12 +69,14 @@ struct fpx_engine {
   int32_t* xch_out = nullptr;          // result of fpx_global_watermark: [1 + kMaxShards]
   // scratch
   uint32_t* bits = nullptr;            // accept / win bitmask, max_batch/32 words
-  int32_t* g_agg = nullptr;            // [kMaxGrid][kMaxKeys] acceptor kernel CTA aggregates
-  uint32_t* g_wacc = nullptr;          // [kMaxGrid*kWarps] accepted per warp range
+  int32_t* g_agg = nullptr;            // [2][kMaxGrid][kMaxKeys] acceptor kernel CTA aggregates
+  uint32_t* g_wacc = nullptr;          // [kAccMaxSegments][kMaxGrid*kAW] accepted per warp range
   uint2* t_bw = nullptr;               // tally: completing-vote bitmap of the running batch + per-word prefix
   uint32_t* t_cc = nullptr;            // tally: completing votes per 1024-vote chunk
   void* t_tmp = nullptr;               // tally: Chosen records parked at their vote's index (max_batch * 8)
   int tally_path = 0;                  // 0 auto, 2 force the exact per-vote path
+  int acc_segments = 0;                // acceptor kernel: 0 = from the batch size and the L2 size, else forced
+  long long l2_bytes = 0;
   void* conflicts = nullptr;           // kMaxConflicts * 8 bytes (acceptor kernel)
   void* arm_conflicts = nullptr;       // kMaxConflicts * 8 bytes (arm kernel)
   uint32_t* arm_bits = nullptr;        // arm kernel: record i created its key, max_batch/32 words
@@ -307,8 +309,8 @@ int fpx_create(fpx_engine** out, const fpx_config* cfg) {
   CKC(cudaMalloc(&e->xch_table, kMaxShards * 8));
   CKC(cudaMalloc(&e->xch_out, (1 + kMaxShards) * 4));
   CKC(cudaMalloc(&e->bits, (mb / 32 + 2) * 4));
-  CKC(cudaMalloc(&e->g_agg, (size_t)kMaxGrid * kMaxKeys * 4));
-  CKC(cudaMalloc(&e->g_wacc, (size_t)kMaxGrid * kAW * 4));
+  CKC(cudaMalloc(&e->g_agg, (size_t)2 * kMaxGrid * kMaxKeys * 4));
+  CKC(cudaMalloc(&e->g_wacc, (size_t)kAccMaxSegments * kMaxGrid * kAW * 4));
   CKC(cudaMalloc(&e->t_bw, (mb / kChunkVotes + 2) * 32 * 8));
   CKC(cudaMalloc(&e->t_cc, (mb / kChunkVotes + 2) * 4));
   CKC(cudaMalloc(&e->t_tmp, (mb + kChunkVotes) * 8));   // padded to a whole chunk: phase D loads unconditionally
@@ -318,11 +320,12 @@ int fpx_create(fpx_engine** out, const fpx_config* cfg) {
     CKC(cudaGetDeviceProperties(&prop, cfg->device));
     if (!prop.cooperativeLaunch) return fail(FPX_ERR_UNSUPPORTED);
     e->num_sms = prop.multiProcessorCount;
+    e->l2_bytes = prop.l2CacheSize;
     int occ = 0;
     CKC(cudaFuncSetAttribute(acceptor_phase2a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             kMaxKeys * kAT * 4));
+                             (kMaxKeys + kAccMaxSegments) * kAT * 4));
     CKC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, acceptor_phase2a_kernel, kAT,
-                                                      (size_t)g.num_keys * kAT * 4));
+                                                      (size_t)(g.num_keys + kAccMaxSegments) * kAT * 4));
     e->occ_acceptor = std::max(occ, 1);
     e->grid_acceptor = std::min(std::max(occ, 1) * e->num_sms, kMaxGrid);
     // the tally's dynamic shared memory: scan of the per-chunk counts (4 B per 1024 votes) + the CTA's kept
@@ -450,6 +453,13 @@ int fpx_debug_set_tally_path(fpx_engine* e, int32_t path) {
   e->tally_path = path;
   return FPX_OK;
 }
+// Undocumented test/profiling aid: cut every acceptor launch into `segments` pipelined segments
+// (1 .. kAccMaxSegments; 0 = automatic, from the batch size and the L2 size).
+int fpx_debug_set_acceptor_segments(fpx_engine* e, int32_t segments) {
+  if (!e || segments < 0 || segments > kAccMaxSegments) return FPX_ERR_INVALID_ARG;
+  e->acc_segments = segments;
+  return FPX_OK;
+}
 int fpx_debug_last_tally_path(fpx_engine* e) {
   if (!e) return FPX_ERR_INVALID_ARG;
   uint32_t v = 0;
@@ -530,12 +540,13 @@ static int acceptor_launch(fpx_engine* e, const fpx_p2a* d_in, int32_t n, fpx_p2
   P.st = e->st;
   P.conflicts = (VoteConflict*)e->conflicts;
   int grid = std::max(1, std::min(e->grid_acceptor, (n + kAT - 1) / kAT));
+  P.segments = e->acc_segments > 0 ? e->acc_segments : acceptor_segments(n, e->l2_bytes);
   P.parity = e->parity;
   P.append = append;
   e->parity ^= 1u;
   void* args[] = {&P};
   CK(e, cudaLaunchCooperativeKernel((const void*)acceptor_phase2a_kernel, dim3(grid), dim3(kAT), args,
-                                    (size_t)e->g.num_keys * kAT * 4, stream));
+                                    (size_t)(e->g.num_keys + P.segments) * kAT * 4, stream));
   e->launches++;
   CK(e, cudaGetLastError());
   return FPX_OK;

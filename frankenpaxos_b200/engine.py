@@ -147,6 +147,10 @@ class Engine:
         """exact=True: every tally launch evaluates each vote (no row sweep)."""
         self._check(self._L.fpx_debug_set_tally_path(self.h, 2 if exact else 0))
 
+    def set_acceptor_segments(self, segments):
+        """Cut every acceptor launch into `segments` pipelined segments (0: automatic, from the L2 size)."""
+        self._check(self._L.fpx_debug_set_acceptor_segments(self.h, segments))
+
     @property
     def last_tally_path(self):
         """'sweep' / 'exact': what the last proxyleader_phase2b launch did."""

@@ -52,6 +52,9 @@ for variant in args.variants.split(","):
     ext = torch.cuda.ExternalStream(eng.stream, device=dev)
     if not args.old_lib:
         eng._check(L.fpx_debug_set_tally_path(eng.h, sum(bit for tok, bit in (("exact", 2), ("nored", 4)) if tok in variant.split("_"))))
+    for tok in variant.split("_"):
+        if tok.startswith("seg"):      # segN: every acceptor launch cut into N pipelined segments (default: from the L2 size)
+            eng.set_acceptor_segments(int(tok[3:]))
     flush = torch.empty(1 << 28, dtype=torch.uint8, device=dev) if "flush" in variant else None
     ins = []
     for s in range(S):
