@@ -3,7 +3,36 @@ oracle with the same delivery trace and compare every observable bit-exactly."""
 import numpy as np
 
 from frankenpaxos_b200 import CHOSEN, NACK, P2A, P2B, Engine, FpxError
+from frankenpaxos_b200 import traces as T
 from oracle import fpx_oracle_py as O
+
+# Quorum systems on both sides of every proxy-leader row size.  A row is {round, value, one stamp per
+# voter} padded to 8, 16 or 32 words, i.e. at most 6, 14 or 30 voters per slot (fpx_create).
+WIDE_SHAPES = {
+    # 7 voters: the smallest 16-word row
+    "maj7": dict(f=3, num_acceptor_groups=1, acceptors_per_group=7, flexible=False, num_leaders=4, num_replicas=4),
+    # 14 voters: a full 16-word row
+    "grid2x7": dict(f=1, num_acceptor_groups=2, acceptors_per_group=7, flexible=True, num_leaders=2, num_replicas=2),
+    # 15 voters: the smallest 32-word row
+    "maj15": dict(f=7, num_acceptor_groups=1, acceptors_per_group=15, flexible=False, num_leaders=8, num_replicas=8),
+    # 15 voters per slot in two groups: 30 acceptors, 32-word rows
+    "groups2x15": dict(f=7, num_acceptor_groups=2, acceptors_per_group=15, flexible=False, num_leaders=8,
+                       num_replicas=8),
+    # 29 voters, 32-word rows
+    "maj29": dict(f=14, num_acceptor_groups=1, acceptors_per_group=29, flexible=False, num_leaders=15,
+                  num_replicas=15),
+    # 30 voters: a full 32-word row
+    "grid5x6": dict(f=1, num_acceptor_groups=5, acceptors_per_group=6, flexible=True, num_leaders=2, num_replicas=2),
+}
+
+
+def voters(cfg):
+    return cfg["num_acceptor_groups"] * cfg["acceptors_per_group"] if cfg["flexible"] else cfg["acceptors_per_group"]
+
+
+def row_words(cfg):
+    v = voters(cfg)
+    return 8 if v <= 6 else (16 if v <= 14 else 32)
 
 
 def make_pair(cfg, slot_capacity, max_batch=1 << 16, overflow_capacity=1 << 8, **kw):
@@ -81,3 +110,39 @@ def compare_acceptors(eng, ora, cfg, first_slot, n_slots):
 
 def compare_log(eng, ora, first_slot, n_slots):
     same(eng.snapshot_log(first_slot, n_slots), ora.snapshot_log(first_slot, n_slots), "replica log")
+
+
+def adversarial(cfg, seed, n_slots, kmax, coop_ctas_per_sm=0, max_batch=1 << 16):
+    """Random rounds (stale and fresh), duplicate deliveries, late votes, several live rounds per slot (so
+    armed rows move to the overflow table), non-thrifty fan-out, many small and large batches; every
+    acceptor and the replica log compared after each phase."""
+    g = T.rng(seed)
+    eng, ora = make_pair(cfg, n_slots, max_batch=max_batch, overflow_capacity=1 << 13 if n_slots <= 3000 else 1 << 20)
+    eng.set_coop_ctas_per_sm(coop_ctas_per_sm)
+    for phase in range(4):
+        k = int(g.integers(1, kmax))
+        slots = g.integers(0, n_slots, size=k).astype(np.int32)
+        rounds = g.integers(0, 4, size=k).astype(np.int32) if phase else np.zeros(k, dtype=np.int32)
+        values = (slots * 8 + rounds).astype(np.int32)   # one value per (slot, round)
+        a = T.arms(slots, 0, values)
+        a["round"] = rounds
+        arm(eng, ora, a)
+        p = T.phase2as(g, slots, cfg["f"], cfg["num_acceptor_groups"], cfg["acceptors_per_group"],
+                       cfg["flexible"], rounds, values, thrifty=bool(g.integers(0, 2)))
+        p = p[g.permutation(len(p))]
+        dup = p[g.integers(0, len(p), size=len(p) // 10)]
+        p = np.concatenate([p, dup])[g.permutation(len(p) + len(dup))]
+        votes = []
+        for chunk in np.array_split(p, int(g.integers(1, 4))):
+            ob, on = phase2a(eng, ora, chunk)
+            votes.append(ob)
+        compare_acceptors(eng, ora, cfg, 0, n_slots)
+        v = np.concatenate(votes)
+        v = np.concatenate([v, v[g.integers(0, max(len(v), 1), size=len(v) // 5)]]) if len(v) else v
+        v = v[g.permutation(len(v))]
+        for chunk in np.array_split(v, int(g.integers(1, 6))):
+            st, c = phase2b(eng, ora, chunk)
+            assert st == 0
+            replica(eng, ora, c)
+    compare_log(eng, ora, 0, n_slots)
+    eng.close()

@@ -18,6 +18,10 @@ SHAPES = {
     "majority3": dict(f=1, num_acceptor_groups=1, acceptors_per_group=3, flexible=False, num_leaders=2, num_replicas=2),
     "grid2x2": dict(f=1, num_acceptor_groups=2, acceptors_per_group=2, flexible=True, num_leaders=2, num_replicas=2),
     "groups2x3": dict(f=1, num_acceptor_groups=2, acceptors_per_group=3, flexible=False, num_leaders=3, num_replicas=2),
+    # 7 voters: a 16-word proxy-leader row
+    "maj7": H.WIDE_SHAPES["maj7"],
+    # a 5 x 6 grid, 30 voters: a full 32-word row
+    "grid5x6": H.WIDE_SHAPES["grid5x6"],
 }
 N_SLOTS = 24
 _engines = {}
@@ -34,11 +38,13 @@ def engine(shape, exact):
 slot = st.integers(0, N_SLOTS - 1)
 rnd = st.integers(0, 3)
 arm_rec = st.tuples(slot, rnd, st.integers(0, 5))
+# group and acceptor indices are drawn from 0..31 and reduced per shape, so that every voter of the widest
+# shape can be drawn
+idx = st.integers(0, 31)
 step = st.one_of(
     st.tuples(st.just("arm"), st.lists(arm_rec, min_size=1, max_size=12)),
-    st.tuples(st.just("p2a"), st.lists(st.tuples(slot, rnd, st.integers(0, 5), st.integers(0, 2), st.integers(0, 3)),
-                                       min_size=1, max_size=40)),
-    st.tuples(st.just("p2b"), st.lists(st.tuples(st.integers(0, 2), st.integers(0, 3), slot, rnd), min_size=1, max_size=40)),
+    st.tuples(st.just("p2a"), st.lists(st.tuples(slot, rnd, st.integers(0, 5), idx, idx), min_size=1, max_size=40)),
+    st.tuples(st.just("p2b"), st.lists(st.tuples(idx, idx, slot, rnd), min_size=1, max_size=40)),
 )
 
 
@@ -47,6 +53,7 @@ step = st.one_of(
 @settings(max_examples=120, deadline=None, suppress_health_check=list(HealthCheck))
 @given(script=st.lists(step, min_size=1, max_size=8))
 def test_fuzz_against_oracle(shape, exact, script):
+    """majority3, grid2x2, groups2x3: 8-word rows; maj7: 16-word rows; grid5x6: 32-word rows."""
     cfg = SHAPES[shape]
     G, A = cfg["num_acceptor_groups"], cfg["acceptors_per_group"]
     eng = engine(shape, exact)
@@ -70,6 +77,8 @@ def test_fuzz_against_oracle(shape, exact, script):
             for g, acc, s, r in recs:
                 if not cfg["flexible"]:
                     g, acc = s % G, acc % A   # in-range ids (precondition); unknown (slot, round) stays possible
+                else:
+                    g, acc = g % (G + 1), acc % (A + 1)   # one row / column past the grid: a foreign voter
                 rows.append((g, acc, s, r))
             stt, c = H.phase2b(eng, ora, np.array(rows, dtype=P2B))
             if stt != 0:

@@ -316,54 +316,26 @@ def test_cfg1_round_bump_nacks():
 
 
 # --------------------------------------------------------------------------- adversarial differential
+NARROW_SHAPES = {
+    "majority5": dict(f=2, num_acceptor_groups=1, acceptors_per_group=5, flexible=False, num_leaders=3, num_replicas=3),
+    "grid2x3": dict(f=1, num_acceptor_groups=2, acceptors_per_group=3, flexible=True, num_leaders=2, num_replicas=2),
+    "groups3x3": dict(f=1, num_acceptor_groups=3, acceptors_per_group=3, flexible=False, num_leaders=2, num_replicas=2),
+}
+SHAPES = {**NARROW_SHAPES, **H.WIDE_SHAPES}
+
+
 @pytest.mark.parametrize("seed", range(6))
-@pytest.mark.parametrize("shape", ["majority5", "grid2x3", "groups3x3"])
+@pytest.mark.parametrize("shape", list(SHAPES))
 def test_adversarial_random_traces(seed, shape):
     """Random rounds (stale and fresh), duplicate deliveries, late votes, several
-    live rounds per slot, non-thrifty fan-out, many small and large batches."""
-    if shape == "majority5":
-        cfg = dict(f=2, num_acceptor_groups=1, acceptors_per_group=5, flexible=False, num_leaders=3,
-                   num_replicas=3)
-    elif shape == "grid2x3":
-        cfg = dict(f=1, num_acceptor_groups=2, acceptors_per_group=3, flexible=True, num_leaders=2,
-                   num_replicas=2)
-    else:
-        cfg = dict(f=1, num_acceptor_groups=3, acceptors_per_group=3, flexible=False, num_leaders=2,
-                   num_replicas=2)
-    _adversarial(cfg, 1000 * seed + len(shape), 3000, 2500)
-
-
-def _adversarial(cfg, seed, n_slots, kmax, coop_ctas_per_sm=0, max_batch=1 << 16):
-    g = T.rng(seed)
-    eng, ora = H.make_pair(cfg, n_slots, max_batch=max_batch, overflow_capacity=1 << 13 if n_slots <= 3000 else 1 << 20)
-    eng.set_coop_ctas_per_sm(coop_ctas_per_sm)
-    for phase in range(4):
-        k = int(g.integers(1, kmax))
-        slots = g.integers(0, n_slots, size=k).astype(np.int32)
-        rounds = g.integers(0, 4, size=k).astype(np.int32) if phase else np.zeros(k, dtype=np.int32)
-        values = (slots * 8 + rounds).astype(np.int32)   # one value per (slot, round)
-        a = T.arms(slots, 0, values)
-        a["round"] = rounds
-        H.arm(eng, ora, a)
-        p = T.phase2as(g, slots, cfg["f"], cfg["num_acceptor_groups"], cfg["acceptors_per_group"],
-                       cfg["flexible"], rounds, values, thrifty=bool(g.integers(0, 2)))
-        p = p[g.permutation(len(p))]
-        dup = p[g.integers(0, len(p), size=len(p) // 10)]
-        p = np.concatenate([p, dup])[g.permutation(len(p) + len(dup))]
-        votes = []
-        for chunk in np.array_split(p, int(g.integers(1, 4))):
-            ob, on = H.phase2a(eng, ora, chunk)
-            votes.append(ob)
-        H.compare_acceptors(eng, ora, cfg, 0, n_slots)
-        v = np.concatenate(votes)
-        v = np.concatenate([v, v[g.integers(0, max(len(v), 1), size=len(v) // 5)]]) if len(v) else v
-        v = v[g.permutation(len(v))]
-        for chunk in np.array_split(v, int(g.integers(1, 6))):
-            st, c = H.phase2b(eng, ora, chunk)
-            assert st == 0
-            H.replica(eng, ora, c)
-    H.compare_log(eng, ora, 0, n_slots)
-    eng.close()
+    live rounds per slot, non-thrifty fan-out, many small and large batches.  Shapes:
+    majority5, grid2x3, groups3x3 (8-word rows); maj7 (7 voters) and grid2x7 (14) on
+    16-word rows; maj15 (15), groups2x15 (15 voters, 30 acceptors), maj29 (29) and
+    grid5x6 (30) on 32-word rows, where the overflow-table move copies up to 30 stamps."""
+    cfg = SHAPES[shape]
+    wide = shape in H.WIDE_SHAPES
+    # a non-thrifty batch of a wide shape carries up to 29 copies per slot
+    H.adversarial(cfg, 1000 * seed + len(shape), 3000, 2500, max_batch=1 << 18 if wide else 1 << 16)
 
 
 @pytest.mark.parametrize("ctas_per_sm", [1, 0])
@@ -372,7 +344,7 @@ def test_results_do_not_depend_on_the_grid_size(ctas_per_sm):
     the same for any grid (fpx_set_coop_ctas_per_sm: engines sharing a GPU run smaller grids).
     Batches of up to 2 * 10^5 records, i.e. more CTAs than one wave at 1 CTA/SM."""
     cfg = dict(f=2, num_acceptor_groups=1, acceptors_per_group=5, flexible=False, num_leaders=3, num_replicas=3)
-    _adversarial(cfg, 4242, 50000, 40000, coop_ctas_per_sm=ctas_per_sm, max_batch=1 << 18)
+    H.adversarial(cfg, 4242, 50000, 40000, coop_ctas_per_sm=ctas_per_sm, max_batch=1 << 18)
 
 
 def test_unknown_key_error_index_is_first_in_order():
@@ -519,12 +491,14 @@ def test_mencius_index_math_and_tally(seed):
 
 
 # --------------------------------------------------------------------------- vanilla Mencius (a9, BASELINE cfg5 shape)
-@pytest.mark.parametrize("f", [1, 3])
+@pytest.mark.parametrize("f", [1, 3, 7])
 def test_vanilla_mencius_matches_oracle(f):
     """cfg5: n = 2f+1 servers, owner = slot % n, the coordinator's own vote is
     pre-seeded, up to n-1 Phase2bs per slot, quorum f+1 (Server.scala:767-829,
     1001-1142).  Also: per-slot round compare (Phase2Nack), Phase2a for an entry that
-    is already chosen, stale / unknown Phase2bs, learn-chosen at other servers."""
+    is already chosen, stale / unknown Phase2bs, learn-chosen at other servers.
+    f = 1: 3 servers, 8-word rows; f = 3: 7 servers, 16-word rows; f = 7: 15 servers,
+    32-word rows (the arm's uint4 stamp rewrite runs over words 4 to 31)."""
     from frankenpaxos_b200 import VANILLA_MENCIUS
     n = 2 * f + 1
     n_slots = 4000
@@ -595,16 +569,13 @@ def test_vanilla_mencius_matches_oracle(f):
 
 
 # --------------------------------------------------------------------------- Phase 1 reads (SURVEY 8(f) rank 2)
-@pytest.mark.parametrize("shape", ["majority5", "grid2x3", "groups3x3"])
+@pytest.mark.parametrize("shape", list(SHAPES))
 def test_phase1a_and_safe_values(shape):
     """Acceptor.handlePhase1a (Acceptor.scala:148-182) and Leader.safeValue
-    (Leader.scala:318-329) over the same vote cells, after traffic in several rounds."""
-    if shape == "majority5":
-        cfg = dict(f=2, num_acceptor_groups=1, acceptors_per_group=5, flexible=False, num_leaders=3, num_replicas=3)
-    elif shape == "grid2x3":
-        cfg = dict(f=1, num_acceptor_groups=2, acceptors_per_group=3, flexible=True, num_leaders=2, num_replicas=2)
-    else:
-        cfg = dict(f=1, num_acceptor_groups=3, acceptors_per_group=3, flexible=False, num_leaders=2, num_replicas=2)
+    (Leader.scala:318-329) over the same vote cells, after traffic in several rounds.
+    Shapes as in test_adversarial_random_traces (8-, 16- and 32-word rows, up to 30
+    acceptors); the responder masks of the wide shapes set acceptor bits 16 to 29."""
+    cfg = SHAPES[shape]
     g = T.rng(len(shape))
     n_slots = 3000
     eng, ora = H.make_pair(cfg, n_slots, overflow_capacity=1 << 13)
@@ -626,7 +597,13 @@ def test_phase1a_and_safe_values(shape):
             exp = [(100 + i, int(vr[i]), int(vv[i])) for i in range(len(vr)) if vr[i] >= 0]
             assert info == exp and r == 7
     H.compare_acceptors(eng, ora, cfg, 0, n_slots)
-    for responders in (0b1, (1 << (G * A)) - 1, 0b101011 & ((1 << (G * A)) - 1), 0):
+    masks = [0b1, (1 << (G * A)) - 1, 0b101011 & ((1 << (G * A)) - 1), 0]
+    if shape in H.WIDE_SHAPES:
+        # responders at and above bit 16 (the second group of groups2x15, the lower rows of grid5x6, the upper
+        # voters of maj29; bits past the last acceptor are ignored), bit 29 alone, every other acceptor, and
+        # a random mask
+        masks += [1 << 29, (1 << 29) | (1 << 16) | 1, 0x3fff0000, 0x2aaaaaaa, int(g.integers(0, 1 << 30))]
+    for responders in masks:
         ev, evv, em = eng.leader_safe_values(responders, 50, 2500)
         ov, ovv, om = ora.safe_values(responders, 50, 2500)
         H.same(ev, ov, "safeValue voteRound"); H.same(evv, ovv, "safeValue value"); assert em == om

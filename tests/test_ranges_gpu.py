@@ -296,8 +296,10 @@ def vm_logs(eng, ora, n, cap):
         assert np.array_equal(vr[pend], r[pend]) and (vr[k == 0] == -1).all()
 
 
-@pytest.mark.parametrize("f", [1, 3])
+@pytest.mark.parametrize("f", [1, 3, 7])
 def test_vanilla_skips_match_oracle(f):
+    """S/vanillamencius Skip: advanceWithSkips at the skipping server and handleSkip elsewhere, against the
+    oracle's logs.  f = 1, 3, 7: 3, 7 and 15 servers, i.e. 8-, 16- and 32-word rows."""
     n = 2 * f + 1
     cap = 40000
     g = T.rng(60 + f)

@@ -7,6 +7,7 @@ fpx_tally.cuh's row sweep evaluates (DESIGN.md section 2); here the rule itself 
 import numpy as np
 import pytest
 
+import harness as H
 from frankenpaxos_b200 import traces as T
 from frankenpaxos_b200.engine import P2B
 from oracle import fpx_oracle_py as O
@@ -25,10 +26,12 @@ def closed_form_chosen(stamps, value, f, flexible, groups, per_group, lo, hi):
     return [(int(s), int(value[s])) for s in order]
 
 
-@pytest.mark.parametrize("name", ["cfg1", "cfg2", "cfg3"])
+@pytest.mark.parametrize("name", ["cfg1", "cfg2", "cfg3", "maj7", "grid2x7", "maj15", "groups2x15", "maj29", "grid5x6"])
 @pytest.mark.parametrize("seed", [0, 1, 2])
 def test_closed_form_completing_vote_matches_the_sequential_handlers(name, seed):
-    cfg, _ = T.config_by_name(name)
+    """cfg1-cfg3: 3, 5 and 6 voters (8-word rows); maj7 and grid2x7: 7 and 14 voters (16-word rows); maj15,
+    groups2x15, maj29 and grid5x6: 15, 15, 29 and 30 voters (32-word rows)."""
+    cfg = H.WIDE_SHAPES[name] if name in H.WIDE_SHAPES else T.config_by_name(name)[0]
     n_slots = 3000
     f, G, A, flexible = cfg["f"], cfg["num_acceptor_groups"], cfg["acceptors_per_group"], cfg["flexible"]
     g = T.rng(700 + seed)
