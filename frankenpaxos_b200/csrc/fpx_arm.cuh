@@ -62,6 +62,22 @@ __device__ __forceinline__ uint32_t* table_insert(const ArmParams& P, int slot, 
   return nullptr;
 }
 
+// fpx_retire_below: linear probing cannot delete, so the table is rebuilt into its spare copy (keys and rows
+// preset to ~0): every key whose slot is still in the live window (g is the geometry after the retire) goes to
+// the first free entry of its probe sequence -- the one table_insert walks -- with its row {header, stamps}
+// copied unchanged; keys of retired slots are dropped.  `used` counts the kept keys.  One thread per entry.
+__global__ void __launch_bounds__(256) ovf_rebuild_kernel(Geometry g, const unsigned long long* keys, const uint32_t* rows,
+                                                           unsigned long long* new_keys, uint32_t* new_rows, uint32_t* used) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= g.ovf_cap) return;
+  const unsigned long long key = keys[i];
+  if (key == kU64Empty || local_slot(g, (int)(key >> 32)) == kLocalRetired) return;
+  uint32_t h = (uint32_t)mix64(key) & g.ovf_mask;
+  while (atomicCAS(&new_keys[h], kU64Empty, key) != kU64Empty) h = (h + 1) & g.ovf_mask;   // never full: same capacity
+  for (int w = 0; w < g.row_words; ++w) new_rows[(size_t)h * g.row_words + w] = rows[(size_t)i * g.row_words + w];
+  atomicAdd(used, 1u);
+}
+
 // second stage of one arm: `old` is what the 64-bit CAS on the primary row's header
 // returned.  Returns true if this record created the key's entry.
 //
@@ -106,12 +122,25 @@ __device__ __forceinline__ bool arm_finish(const ArmParams& P, const int4& rec, 
       return false;
     }
     t[0] = orw;
+    // the slot's first key entered the table: it is no longer empty (DevStatus::ovf_used).  Counted here and
+    // not per insert -- every key of the table belongs to a moved slot, and this spot adds no register pressure
+    red_add_u32(&P.st->ovf_used, 1u);
     t[1] = (uint32_t)(old >> 32);
     for (int v = 0; v < g.voters; ++v) t[2 + v] = prim[2 + v];
     __threadfence();
     old = (old & 0xffffffff00000000ull) | kPoison;
     atomicExch(hdr, old);
   }
+}
+
+// Server.handleClientRequest for a slot retired by fpx_retire_below: the owner's entry is a ChosenEntry, so
+// the request is dropped (phase2s / log already hold the slot, :773-774) once it passes the checks a live
+// slot's request passes first.
+__device__ __forceinline__ void vm_retired_request(const ArmParams& P, const int4& rec, int i) {
+  const Geometry& g = P.g;
+  if ((uint32_t)rec.y > (uint32_t)FPX_MAX_ROUND || rec.y != 0) report_error(P.st, FPX_ERR_ROUND_RANGE, i);
+  else if ((rec.w >> 16) != 0 || (rec.w & 0xffff) >= g.per_group || rec.x % g.per_group != (rec.w & 0xffff))
+    report_error(P.st, FPX_ERR_BAD_ACCEPTOR, i);
 }
 
 constexpr int kArmUnroll = 8;
@@ -129,7 +158,7 @@ __device__ __forceinline__ int arm_chunks(const ArmParams& P, int gwarp, int tot
   for (int c0 = gwarp * kArmUnroll; c0 < n_chunks; c0 += total_warps * kArmUnroll) {
     unsigned long long old[kArmUnroll];
     unsigned long long want[kArmUnroll];
-    int local[kArmUnroll];          // row of the record, -1: not a valid arm
+    int local[kArmUnroll];          // row of the record, -1: not a valid arm, kLocalRetired: vanilla, retired slot
     {
       int4 rec[kArmUnroll];
 #pragma unroll
@@ -146,6 +175,7 @@ __device__ __forceinline__ int arm_chunks(const ArmParams& P, int gwarp, int tot
           int l = local_slot(g, rec[u].x);
           if (l < 0) {
             if (l != kLocalRetired) report_error(P.st, FPX_ERR_SLOT_RANGE, i);   // retired: the key is Done, `case Some(_)` (:177-183)
+            else if (P.vanilla) vm_retired_request(P, rec[u], i);
           } else if ((uint32_t)rec[u].y > (uint32_t)FPX_MAX_ROUND) {
             report_error(P.st, FPX_ERR_ROUND_RANGE, i);
           } else if (P.vanilla && rec[u].y != 0) {

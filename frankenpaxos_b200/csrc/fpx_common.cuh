@@ -46,7 +46,7 @@ struct DevStatus {
   uint32_t n_conflicts;         // entries in the conflict list of the running call
   uint32_t ticket;              // last-block-done ticket
   int32_t wm_local;             // replica: first local index not yet chosen
-  int32_t max_chosen_local;     // replica: largest local index ever chosen
+  int32_t max_chosen_local;     // replica: largest ordinal (slot / shard_count) ever chosen
   int32_t wm_found;             // scratch of the watermark scan
   uint32_t bar_count;           // grid barrier: CTAs arrived at the running barrier (self-resetting)
   uint32_t nack_total;          // acceptor kernel: Nacks of the running call
@@ -62,6 +62,11 @@ struct DevStatus {
   uint32_t wm_need_scan;                // fused tally: the sweep could not settle the watermark, run the first-hole scan
   unsigned long long t_acceptor[8];  // %globaltimer at the phase boundaries of CTA 0 (profiling aid)
   unsigned long long t_tally[8];
+  // zero iff the key table is empty; fpx_retire_below rebuilds a table only while its count is non-zero
+  uint32_t ovf_used;                    // overflow (slot, round) table: keys the last rebuild kept + slots moved
+                                        // into the table since (a moved slot's first key; its later keys share
+                                        // the slot, so they leave with it)
+  uint32_t rng_used;                    // mencius noop-range table: occupied entries
 };
 
 __device__ __forceinline__ unsigned long long global_timer_ns() {
@@ -183,6 +188,9 @@ __device__ __forceinline__ unsigned long long ld_u64_evict_last(const unsigned l
 // `red` is the fire-and-forget form (REDG).
 __device__ __forceinline__ void red_min_u32(uint32_t* p, uint32_t v) {
   asm volatile("red.global.min.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ void red_add_u32(uint32_t* p, uint32_t v) {
+  asm volatile("red.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ void red_or_u32(uint32_t* p, uint32_t v) {
   asm volatile("red.global.or.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory");

@@ -44,12 +44,15 @@ struct fpx_engine {
   uint32_t* rows = nullptr;
   unsigned long long* ovf_keys = nullptr;
   uint32_t* ovf_rows = nullptr;
+  unsigned long long* ovf_keys_spare = nullptr;   // fpx_retire_below rebuilds the overflow table into these and swaps
+  uint32_t* ovf_rows_spare = nullptr;
   unsigned long long* votes = nullptr;
   int32_t* acc_round = nullptr;
   int32_t* acc_max_voted = nullptr;
   unsigned long long* rlog = nullptr;
   uint32_t vm_tag = 1;
   uint32_t* rng_tab = nullptr;             // mencius: (start, end, round) key table of the NoopRange path
+  uint32_t* rng_tab_spare = nullptr;       // its rebuild target (fpx_retire_below)
   int32_t rng_cap = 0;
   int32_t* rng_dec = nullptr;              // per-record scratch of the range kernels (FPX_MAX_RANGE_BATCH)
   uint32_t rng_seq_base = 1;               // Phase2bNoopRange delivery sequence numbers
@@ -294,6 +297,8 @@ int fpx_create(fpx_engine** out, const fpx_config* cfg) {
   if (g.ovf_cap) {
     CKC(cudaMalloc(&e->ovf_keys, (size_t)g.ovf_cap * 8));
     CKC(cudaMalloc(&e->ovf_rows, (size_t)g.ovf_cap * g.row_words * 4));
+    CKC(cudaMalloc(&e->ovf_keys_spare, (size_t)g.ovf_cap * 8));
+    CKC(cudaMalloc(&e->ovf_rows_spare, (size_t)g.ovf_cap * g.row_words * 4));
   }
   CKC(cudaMalloc(&e->votes, ((size_t)g.local_slots * g.voters * 8) << g.cell_shift));
   CKC(cudaMalloc(&e->acc_round, kMaxKeys * 4));
@@ -302,6 +307,7 @@ int fpx_create(fpx_engine** out, const fpx_config* cfg) {
   if (cfg->protocol == FPX_MENCIUS) {
     e->rng_cap = std::max(1024, g.ovf_cap);
     CKC(cudaMalloc(&e->rng_tab, (size_t)e->rng_cap * kRangeWords * 4));
+    CKC(cudaMalloc(&e->rng_tab_spare, (size_t)e->rng_cap * kRangeWords * 4));
   }
   if (cfg->protocol != FPX_MULTIPAXOS) CKC(cudaMalloc(&e->rng_dec, (size_t)(FPX_MAX_RANGE_BATCH + 1) * 4));
   CKC(cudaMalloc(&e->st, sizeof(DevStatus)));
@@ -364,8 +370,9 @@ void fpx_destroy(fpx_engine* e) {
   cudaSetDevice(e->cfg.device);
   if (e->stream) cudaStreamSynchronize(e->stream);
   cudaFree(e->rows); cudaFree(e->ovf_keys); cudaFree(e->ovf_rows); cudaFree(e->votes);
+  cudaFree(e->ovf_keys_spare); cudaFree(e->ovf_rows_spare);
   cudaFree(e->acc_round); cudaFree(e->acc_max_voted); cudaFree(e->rlog); cudaFree(e->st);
-  cudaFree(e->rng_tab); cudaFree(e->rng_dec);
+  cudaFree(e->rng_tab); cudaFree(e->rng_tab_spare); cudaFree(e->rng_dec);
   for (auto& ln : e->lane) {
     cudaFree(ln.d_p2a); cudaFree(ln.d_p2b); cudaFree(ln.d_arm); cudaFree(ln.d_out_p2b); cudaFree(ln.d_out_nack); cudaFree(ln.d_out_chosen);
     for (cudaEvent_t ev : {ln.ev_p2a, ln.ev_p2b, ln.ev_acc, ln.ev_done, ln.ev_d2h}) if (ev) cudaEventDestroy(ev);
@@ -402,10 +409,38 @@ void* fpx_stream(fpx_engine* e) { return e ? (void*)e->stream : nullptr; }
 // published) and will not be needed again -- its row, vote cells and log entry are recycled for the slots
 // slot_capacity ahead.  Messages for retired slots afterwards behave as the reference's would on a key that is
 // Done / a log entry that exists: arms, votes and Chosen records are ignored, a Phase2a is still answered
-// (round compare, Phase2b / Nack) but not recorded.
+// (round compare, Phase2b / Nack) but not recorded.  Vanilla Mencius answers it with reply kind 3.
+// The key tables (secondary (slot, round) keys, mencius noop ranges) drop the keys of retired slots: each is
+// rebuilt into its spare copy and the two are swapped -- kernels take PLState / RangeTable by value at launch,
+// and every earlier launch has finished (fpx_sync).  A table that holds no key (the count the insert paths keep
+// in the status block, read by that same sync) is left alone, so the steady state costs one recycle_kernel.
+static int rebuild_tables(fpx_engine* e) {
+  const Geometry& g = e->g;
+  if (g.ovf_cap && e->h_st->ovf_used != 0) {
+    CK(e, cudaMemsetAsync(e->ovf_keys_spare, 0xff, (size_t)g.ovf_cap * 8, e->stream));
+    CK(e, cudaMemsetAsync(e->ovf_rows_spare, 0xff, (size_t)g.ovf_cap * g.row_words * 4, e->stream));
+    CK(e, cudaMemsetAsync(&e->st->ovf_used, 0, 4, e->stream));
+    ovf_rebuild_kernel<<<(g.ovf_cap + 255) / 256, 256, 0, e->stream>>>(g, e->ovf_keys, e->ovf_rows, e->ovf_keys_spare,
+                                                                      e->ovf_rows_spare, &e->st->ovf_used);
+    e->launches++;
+    CK(e, cudaGetLastError());
+    std::swap(e->ovf_keys, e->ovf_keys_spare);
+    std::swap(e->ovf_rows, e->ovf_rows_spare);
+  }
+  if (e->rng_tab && e->h_st->rng_used != 0) {
+    CK(e, cudaMemsetAsync(e->rng_tab_spare, 0xff, (size_t)e->rng_cap * kRangeWords * 4, e->stream));
+    CK(e, cudaMemsetAsync(&e->st->rng_used, 0, 4, e->stream));
+    range_rebuild_kernel<<<(e->rng_cap + 255) / 256, 256, 0, e->stream>>>(
+        g, RangeTable{e->rng_tab, (uint32_t)e->rng_cap - 1u, e->rng_cap}, e->rng_tab_spare, &e->st->rng_used);
+    e->launches++;
+    CK(e, cudaGetLastError());
+    std::swap(e->rng_tab, e->rng_tab_spare);
+  }
+  return FPX_OK;
+}
+
 int fpx_retire_below(fpx_engine* e, int32_t slot) {
   if (!e || slot < 0) return FPX_ERR_INVALID_ARG;
-  if (e->g.protocol == FPX_VANILLA_MENCIUS) return FPX_ERR_UNSUPPORTED;   // a retired ChosenEntry must still answer Chosen(value)
   CK(e, cudaSetDevice(e->cfg.device));
   fpx_sync_result r;
   int c = fpx_sync(e, &r);
@@ -424,7 +459,7 @@ int fpx_retire_below(fpx_engine* e, int32_t slot) {
   g.base_ring = (int32_t)(new_base % g.local_slots);
   long long cap = (long long)e->cfg.slot_capacity + (long long)g.base_local * g.shard_count;
   g.slot_capacity = (int32_t)std::min<long long>(cap, 0x7fffffffll);
-  return FPX_OK;
+  return rebuild_tables(e);
 }
 
 int fpx_set_coop_ctas_per_sm(fpx_engine* e, int32_t ctas_per_sm) {

@@ -54,8 +54,8 @@ __device__ __forceinline__ uint32_t* range_find(const RangeTable& t, int start, 
   }
   return nullptr;
 }
-// insert-if-absent; returns nullptr when the table is full
-__device__ __forceinline__ uint32_t* range_insert(const RangeTable& t, int start, int end, int round) {
+// insert-if-absent; returns nullptr when the table is full.  *used counts the occupied entries.
+__device__ __forceinline__ uint32_t* range_insert(const RangeTable& t, int start, int end, int round, uint32_t* used) {
   uint32_t h = range_hash(start, end, round) & t.mask;
   for (int probe = 0; probe < t.cap; ++probe) {
     uint32_t* e = t.ent + (size_t)h * kRangeWords;
@@ -64,6 +64,7 @@ __device__ __forceinline__ uint32_t* range_insert(const RangeTable& t, int start
       e[1] = (uint32_t)start; e[2] = (uint32_t)end; e[3] = (uint32_t)round;
       __threadfence();
       atomicExch(e, kRangePending);
+      red_add_u32(used, 1u);
       return e;
     }
     while (s == kRangeBusy) s = *(volatile uint32_t*)e;
@@ -72,6 +73,28 @@ __device__ __forceinline__ uint32_t* range_insert(const RangeTable& t, int start
     h = (h + 1) & t.mask;
   }
   return nullptr;
+}
+
+// A non-empty range that lies below base_local * shard_count: every slot of it that this shard holds was
+// retired by fpx_retire_below (with one shard: every slot of it).  Its key is Done for good -- it leaves the
+// table at the next retire and a late arm does not bring it back.
+__device__ __forceinline__ bool range_retired(const Geometry& g, int start, int end) {
+  return start < end && (long long)end <= (long long)g.base_local * g.shard_count;
+}
+
+// fpx_retire_below: the range table rebuilt into its spare copy (preset to ~0), like ovf_rebuild_kernel: the
+// entries of ranges that are not retired under the new geometry g move, whole, to the first free entry of
+// their probe sequence; `used` counts them.  One thread per entry.
+__global__ void __launch_bounds__(256) range_rebuild_kernel(Geometry g, RangeTable from, uint32_t* to, uint32_t* used) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= from.cap) return;
+  const uint32_t* e = from.ent + (size_t)i * kRangeWords;
+  const uint32_t state = e[0];
+  if (state == kRangeEmpty || range_retired(g, (int)e[1], (int)e[2])) return;
+  uint32_t h = range_hash((int)e[1], (int)e[2], (int)e[3]) & from.mask;
+  while (atomicCAS(to + (size_t)h * kRangeWords, kRangeEmpty, state) != kRangeEmpty) h = (h + 1) & from.mask;
+  for (int w = 1; w < kRangeWords; ++w) to[(size_t)h * kRangeWords + w] = e[w];
+  atomicAdd(used, 1u);
 }
 
 __device__ __forceinline__ int range_precheck(const Geometry& g, int start, int end, int round) {
@@ -108,11 +131,12 @@ __global__ void __launch_bounds__(256) range_arm_kernel(RangeArmParams P) {
     int4 rec = P.in[i];
     int c = range_precheck(g, rec.x, rec.y, rec.z);
     if (c != FPX_OK) { report_error(P.st, c, i); continue; }
+    if (range_retired(g, rec.x, rec.y)) continue;   // the key is Done (or was never needed): `case Some(_)`
     if (rec.y == rec.x + 1) {
       int l = local_slot(g, rec.x);
       if (l >= 0 && find_row(g, P.pl, l, rec.x, rec.z).p != nullptr) continue;   // `case Some(_)`
     }
-    if (range_insert(P.tab, rec.x, rec.y, rec.z) == nullptr) report_error(P.st, FPX_ERR_OVERFLOW_FULL, i);
+    if (range_insert(P.tab, rec.x, rec.y, rec.z, &P.st->rng_used) == nullptr) report_error(P.st, FPX_ERR_OVERFLOW_FULL, i);
   }
 }
 
@@ -273,8 +297,10 @@ __global__ void __launch_bounds__(kRangeCtaThreads) range_tally_kernel(RangeTall
   for (int i = tid; i < P.n; i += kRangeCtaThreads) {
     const int4 rec = P.in[i];
     int d = 0;
-    uint32_t* e = range_find(P.tab, rec.y, rec.z, rec.w);
-    if (e == nullptr) {
+    uint32_t* e = nullptr;
+    if (range_retired(g, rec.y, rec.z)) {
+      // a retired range was chosen long ago: the vote finds `Done` and is ignored (:372-388)
+    } else if ((e = range_find(P.tab, rec.y, rec.z, rec.w)) == nullptr) {
       bool single = false;
       if (rec.z == rec.y + 1) {
         int l = local_slot(g, rec.y);
@@ -367,7 +393,8 @@ __global__ void __launch_bounds__(256) replica_range_first_kernel(ReplicaRangePa
        t += (long long)gridDim.x * blockDim.x) {
     int slot = (int)(rec.x + t * LG);
     int l = local_slot(g, slot);
-    if (l >= 0 && __ldcg(&P.rlog[l]) != kU64Empty) hit = slot;   // ascending per thread: first hit is its minimum
+    // ascending per thread: first hit is its minimum.  A retired slot is in the log (executed long ago).
+    if (l == kLocalRetired || (l >= 0 && __ldcg(&P.rlog[l]) != kU64Empty)) hit = slot;
   }
   hit = __reduce_min_sync(0xffffffffu, hit);
   if ((threadIdx.x & 31) == 0 && hit != kNoHit) atomicMin(&P.first[j], hit);
@@ -389,7 +416,7 @@ __global__ void __launch_bounds__(256) replica_range_fill_kernel(ReplicaRangePar
                                                        (uint32_t)FPX_VALUE_NOOP);
     if (old != kU64Empty)   // another record of this call covers the slot too: the later of the two is at fault
       report_error(P.st, FPX_ERR_BATCH_ORDER, max((long long)j, (long long)(uint32_t)(old >> 32) - (long long)P.seq_base));
-    mx = max(mx, l);
+    mx = max(mx, g.base_local + ring_to_rel(g, l));   // an ordinal, like every other writer of max_chosen_local
   }
   mx = __reduce_max_sync(0xffffffffu, mx);
   if ((threadIdx.x & 31) == 0 && mx != INT_MIN) atomicMax(&P.st->max_chosen_local, mx);
@@ -431,7 +458,11 @@ __global__ void __launch_bounds__(256) vm_skip_kernel(VmSkipParams P) {
   for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < count; t += (long long)gridDim.x * blockDim.x) {
     const int slot = (int)(rec.y + t * n);
     const int l = local_slot(g, slot);
-    if (l < 0) continue;
+    if (l < 0) {
+      // retired: a ChosenEntry at every server -- not vacant for the fill (:613-614), already chosen for handleSkip
+      if (l == kLocalRetired && rec.w) report_error(P.st, FPX_ERR_CHECK_FAILED, j);
+      continue;
+    }
     unsigned long long* cell = &P.votes[cell_index(g, l, server)];
     uint32_t* row = P.rows + (size_t)l * g.row_words;
     if (rec.w) {

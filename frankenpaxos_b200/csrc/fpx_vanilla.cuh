@@ -91,9 +91,13 @@ __global__ void __launch_bounds__(256, 3) vm_phase2a_kernel(VmParams P) {
       if (i >= P.n) continue;
       const int server = rec[u].w & 0xffff;
       const int local = local_slot(g, rec[u].x);
-      if (local < 0) { report_error(P.st, FPX_ERR_SLOT_RANGE, i); continue; }
-      if ((rec[u].w >> 16) != 0 || server >= g.per_group) { report_error(P.st, FPX_ERR_BAD_ACCEPTOR, i); continue; }
-      if ((uint32_t)rec[u].y > (uint32_t)FPX_MAX_ROUND) { report_error(P.st, FPX_ERR_ROUND_RANGE, i); continue; }
+      int c = local == -1 ? FPX_ERR_SLOT_RANGE
+              : ((rec[u].w >> 16) != 0 || server >= g.per_group) ? FPX_ERR_BAD_ACCEPTOR
+              : (uint32_t)rec[u].y > (uint32_t)FPX_MAX_ROUND ? FPX_ERR_ROUND_RANGE : FPX_OK;
+      if (c != FPX_OK) { report_error(P.st, c, i); continue; }
+      // kLocalRetired (fpx_retire_below): the entry is a ChosenEntry whose value is the shared log's executed
+      // entry -- the reference's Chosen(slot, value), :1016-1025, without the value
+      if (local < 0) { rk[u] = FPX_VM_REPLY_CHOSEN_RETIRED; continue; }
       cellp[u] = P.votes + cell_index(g, local, server);
       asm volatile("ld.global.cg.v2.u64 {%0,%1}, [%2];" : "=l"(pre0[u]), "=l"(pre1[u]) : "l"(cellp[u]));
     }
@@ -139,8 +143,9 @@ __global__ void __launch_bounds__(256) vm_learn_chosen_kernel(VmParams P) {
   int4 rec = P.in[i];
   int server = rec.y, slot = rec.z;
   int local = local_slot(g, slot);
-  if (local < 0) { report_error(P.st, FPX_ERR_SLOT_RANGE, i); return; }
+  if (local < 0 && local != kLocalRetired) { report_error(P.st, FPX_ERR_SLOT_RANGE, i); return; }
   if ((uint32_t)server >= (uint32_t)g.per_group) { report_error(P.st, FPX_ERR_BAD_ACCEPTOR, i); return; }
+  if (local == kLocalRetired) return;   // retired: every server's entry is a ChosenEntry already, nothing to learn
   red_max_u64(&P.votes[cell_index(g, local, server)], kCellChosen | (uint32_t)rec.w);   // ChosenEntry (:624)
   if (slot % g.per_group == server) {                                                       // phase2s.remove(slot) (:625)
     uint32_t* row = P.rows + (size_t)local * g.row_words;

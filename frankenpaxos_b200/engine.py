@@ -24,6 +24,8 @@ WIRE_PROXYLEADER_INBOUND, WIRE_ACCEPTOR_INBOUND = 0, 1
 WIRE_MENCIUS_PROXYLEADER_INBOUND, WIRE_MENCIUS_ACCEPTOR_INBOUND = 2, 3
 
 MULTIPAXOS, MENCIUS, VANILLA_MENCIUS = 0, 1, 2
+# reply kinds of Engine.vm_phase2a (include/fpx.h FPX_VM_REPLY_*)
+VM_REPLY_PHASE2B, VM_REPLY_NACK, VM_REPLY_CHOSEN, VM_REPLY_CHOSEN_RETIRED = 0, 1, 2, 3
 
 OK = 0
 ERR_INVALID_ARG, ERR_CONFIG, ERR_CUDA, ERR_UNKNOWN_SLOT_ROUND, ERR_BAD_ACCEPTOR = -1, -2, -3, -4, -5
@@ -97,7 +99,10 @@ class Engine:
         self._check(self._L.fpx_reset(self.h))
 
     def retire_below(self, slot):
-        """Slide the live window: slots below `slot` (all executed) are recycled for the slots slot_capacity ahead."""
+        """Slide the live window: slots below `slot` (all executed) are recycled for the slots slot_capacity ahead.
+        Secondary (slot, round) keys and Mencius noop-range keys of retired slots leave their tables, so
+        leader changes and lagging leader groups do not fill them up.  All three protocols; with vanilla
+        Mencius a Phase2a for a retired slot is answered with reply kind VM_REPLY_CHOSEN_RETIRED."""
         self._check(self._L.fpx_retire_below(self.h, slot))
 
     def _check(self, st, idx=-1):
@@ -241,7 +246,8 @@ class Engine:
         self._check(self._L.fpx_vm_client_request(self.h, p2a.ctypes.data, len(p2a), C.byref(err)), err.value)
 
     def vm_phase2a(self, p2a):
-        """dense replies {group = kind (0 Phase2b, 1 Phase2Nack, 2 Chosen), acceptor = server, slot, round|value}"""
+        """dense replies {group = kind (0 Phase2b, 1 Phase2Nack, 2 Chosen, 3 Chosen of a retired slot whose value
+        is the shared log's executed entry), acceptor = server, slot, round|value (0 for kind 3)}"""
         p2a = np.ascontiguousarray(p2a, dtype=P2A)
         out = np.empty(max(len(p2a), 1), dtype=P2B)
         err = C.c_int64(-1)

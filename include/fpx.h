@@ -140,7 +140,11 @@ typedef struct {
   int32_t num_replicas;
   int32_t slot_capacity;        /* GLOBAL slots [0, slot_capacity) the log can hold      */
   int32_t overflow_capacity;    /* secondary (slot, round) keys (two live rounds of one
-                                   slot after a leader change); power of two or 0        */
+                                   slot after a leader change); power of two or 0.  The
+                                   table is held twice (fpx_retire_below rebuilds it into
+                                   the spare copy): 2 x capacity x (8 + 4 x row words)
+                                   bytes; FPX_MENCIUS also holds its noop-range table
+                                   of max(1024, capacity) keys twice                     */
   int32_t max_batch;            /* largest n of any one call                             */
   int32_t device;               /* CUDA ordinal                                          */
   int32_t shard_index;          /* this engine owns slots with slot % shard_count ==     */
@@ -283,7 +287,13 @@ int fpx_vm_client_request(fpx_engine* e, const fpx_p2a* in, int32_t n, int64_t* 
  * answers in[i]: {group = kind, acceptor = server, slot, round}:
  *   kind 0  Phase2b(server, slot, round)                 (:1077-1081)
  *   kind 1  Phase2Nack(slot, round = the entry's round)  (:1044-1051)
- *   kind 2  Chosen(slot, value in `round`)               (:1018-1027, entry already chosen) */
+ *   kind 2  Chosen(slot, value in `round`)               (:1018-1027, entry already chosen)
+ *   kind 3  {3, server, slot, 0}: the slot was retired by fpx_retire_below.  The reference answers
+ *           Chosen(slot, value) (:1016-1025), but the engine no longer holds the value: it is the
+ *           shared log's executed entry of the slot, which the caller holds.  This is the one reply
+ *           that differs from the reference's; a server that had not learned the slot before it was
+ *           retired would have answered Phase2b or Phase2Nack there, and gets kind 3 here as well. */
+enum { FPX_VM_REPLY_PHASE2B = 0, FPX_VM_REPLY_NACK = 1, FPX_VM_REPLY_CHOSEN = 2, FPX_VM_REPLY_CHOSEN_RETIRED = 3 };
 int fpx_vm_phase2a(fpx_engine* e, const fpx_p2a* in, int32_t n, fpx_p2b* reply, int64_t* err_index);
 /* device-pointer forms (asynchronous on the engine's stream, errors surface at fpx_sync) */
 int fpx_vm_client_request_dev(fpx_engine* e, const fpx_p2a* d_in, int32_t n);
@@ -639,8 +649,16 @@ int fpx_global_watermark(fpx_engine* e, uint32_t epoch, int32_t timeout_ms, int3
  * reference's would: an arm / vote / Chosen finds the key Done or the entry present and is ignored; a Phase2a
  * is answered (round compare, Phase2b or Nack) but the vote is not recorded -- Phase1b never reads below the
  * chosen watermark (Acceptor.scala:171-179).  Slots at or beyond base + slot_capacity are FPX_ERR_SLOT_RANGE.
- * Secondary (slot, round) keys of retired slots stay in the overflow table until fpx_reset.  Not offered for
- * FPX_VANILLA_MENCIUS (a retired ChosenEntry would have to answer with its value). */
+ * Secondary (slot, round) keys of retired slots leave the overflow table, so an engine survives any number of
+ * leader changes; the table is rebuilt only while it holds keys, otherwise a retire is one kernel launch.
+ * FPX_MENCIUS: a Phase2aNoopRange key leaves its table once the range lies below base_local * shard_count
+ * (every slot of the range that this shard holds is retired); a later arm of such a range is ignored and not
+ * armed again, a later Phase2bNoopRange is ignored like one for a Done key.  Ranges that reach into the live
+ * window keep their key.
+ * FPX_VANILLA_MENCIUS: every server's entry of a retired slot counts as a ChosenEntry whose value the engine
+ * no longer holds.  A Phase2a gets reply kind 3 (FPX_VM_REPLY_CHOSEN_RETIRED, see fpx_vm_phase2a); a Phase2b,
+ * fpx_vm_learn_chosen and an own = 0 skip are ignored; an own = 1 skip is FPX_ERR_CHECK_FAILED (the slot is
+ * not vacant); a client request is ignored (the reference's check(!log.contains) drops a duplicate). */
 int fpx_retire_below(fpx_engine* e, int32_t slot);
 
 /* The engine's CUDA stream (a cudaStream_t) so a caller can order its own work
