@@ -50,7 +50,8 @@ struct CiParams {
 
 constexpr int32_t kCiEmptyKey = INT32_MIN;
 
-// (1) deps_out = snapshots; rows of every access (one thread per command: commands carry few keys)
+// (1) deps_out = snapshots; rows of every access (one thread per command: commands carry few keys).  acc_row
+//     arrives all kCiNoRow (memset by the host), so a rejected command's accesses have no row.
 __global__ void ci_rows_kernel(CiParams P) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= P.n_cmd) return;

@@ -108,12 +108,13 @@ __global__ void __launch_bounds__(kDgThreads, 1) dg_execute_kernel(DgState S) {
   const int t0 = blockIdx.x * kDgThreads + threadIdx.x;
   int round = 0;
   if (t0 == 0) { S.flags[0] = 0; S.flags[1] = 0; S.flags[2] = 0; S.flags[3] = 0; }
-  // ---- eligibility, seed: a dependency that is neither committed nor executed blocks (:386-392)
+  // ---- eligibility, seed: a dependency that is neither committed nor executed blocks (:386-392).
+  // `blocker` is cleared by the host before the launch: vertex w's flag is set by whichever thread owns a
+  // vertex depending on w, possibly in an earlier stride iteration than the one that reaches w.
   for (int v = t0; v < S.cap; v += stride) {
     S.comp[v] = -1;
     S.mark[v] = 0;
     S.level[v] = kDgNoLevel;
-    S.blocker[v] = 0;
     uint8_t bad = 0;
     if (S.status[v] == kDgCommitted) {
       for (int d = 0; d < S.dep_cnt[v]; ++d) {
