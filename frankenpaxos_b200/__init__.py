@@ -12,4 +12,7 @@ from .engine import (CHOSEN, NACK, P2A, P2B, Engine, FpxError, dst,  # noqa: F40
                      WIRE_REC, WIRE_PROXYLEADER_INBOUND, WIRE_ACCEPTOR_INBOUND,
                      WIRE_MENCIUS_PROXYLEADER_INBOUND, WIRE_MENCIUS_ACCEPTOR_INBOUND)
 
-__all__ = ["Engine", "FpxError", "P2A", "P2B", "CHOSEN", "NACK", "dst"]
+from .reads import (Reads, READS_CLIENT, READS_READ_BATCHER, READ_OPEN, MAX_SLOT_REPLY, READ_SLOT,  # noqa: F401
+                    READ_REQUEST, READ_REPLY)
+
+__all__ = ["Engine", "FpxError", "P2A", "P2B", "CHOSEN", "NACK", "dst", "Reads"]

@@ -32,6 +32,8 @@ SYMBOLS = [
     "fpx_epaxos_preacceptok_dev", "fpx_epaxos_acceptok_dev", "fpx_epaxos_preaccept_sets",
     "fpx_epaxos_create", "fpx_epaxos_destroy", "fpx_epaxos_lead", "fpx_epaxos_preaccept", "fpx_epaxos_accept",
     "fpx_epaxos_preacceptok", "fpx_epaxos_acceptok", "fpx_epaxos_entry", "fpx_epaxos_last_kernel_ms", "fpx_depset_union", "fpx_depset_union_dense_dev",
+    "fpx_reads_create", "fpx_reads_destroy", "fpx_reads_open", "fpx_reads_max_slot_replies", "fpx_reads_replica",
+    "fpx_reads_advance", "fpx_reads_max_slot_replies_dev", "fpx_reads_replica_dev", "fpx_reads_advance_dev", "fpx_reads_sync",
 ]
 
 
@@ -48,6 +50,12 @@ class SyncResult(C.Structure):
     _fields_ = [("status", C.c_int32), ("reserved", C.c_int32), ("err_index", C.c_int64),
                 ("n_p2b", C.c_int32), ("n_nack", C.c_int32), ("n_chosen", C.c_int32),
                 ("watermark", C.c_int32)]
+
+
+class ReadsSyncResult(C.Structure):
+    """struct fpx_reads_sync_result (include/fpx.h)."""
+    _fields_ = [("status", C.c_int32), ("watermark", C.c_int32), ("err_index", C.c_int64),
+                ("n_slots", C.c_int32), ("n_replies", C.c_int32), ("n_released", C.c_int32), ("n_pending", C.c_int32)]
 
 
 def lib():
@@ -126,6 +134,16 @@ def lib():
     L.fpx_exchange_epoch.argtypes = [vp]; L.fpx_exchange_epoch.restype = C.c_uint32
     L.fpx_global_watermark_dev.argtypes = [vp, C.c_uint32, i32, vp, vp]; L.fpx_global_watermark_dev.restype = i32
     L.fpx_global_watermark.argtypes = [vp, C.c_uint32, i32, p(i32), vp]; L.fpx_global_watermark.restype = i32
+    L.fpx_reads_create.argtypes = [p(vp), vp, i32, i32, i32, i32]; L.fpx_reads_create.restype = i32
+    L.fpx_reads_destroy.argtypes = [vp]; L.fpx_reads_destroy.restype = None
+    L.fpx_reads_open.argtypes = [vp, vp, i32, p(i64)]; L.fpx_reads_open.restype = i32
+    L.fpx_reads_max_slot_replies.argtypes = [vp, vp, i32, vp, p(i32), p(i64)]; L.fpx_reads_max_slot_replies.restype = i32
+    L.fpx_reads_replica.argtypes = [vp, vp, i32, vp, p(i32), p(i64)]; L.fpx_reads_replica.restype = i32
+    L.fpx_reads_advance.argtypes = [vp, i32, vp, p(i32)]; L.fpx_reads_advance.restype = i32
+    L.fpx_reads_max_slot_replies_dev.argtypes = [vp, vp, i32, vp]; L.fpx_reads_max_slot_replies_dev.restype = i32
+    L.fpx_reads_replica_dev.argtypes = [vp, vp, i32, vp]; L.fpx_reads_replica_dev.restype = i32
+    L.fpx_reads_advance_dev.argtypes = [vp, vp, vp]; L.fpx_reads_advance_dev.restype = i32
+    L.fpx_reads_sync.argtypes = [vp, p(ReadsSyncResult)]; L.fpx_reads_sync.restype = i32
     if hasattr(L, "fpx_debug_set_tally_path"):
         L.fpx_debug_set_tally_path.argtypes = [vp, i32]; L.fpx_debug_set_tally_path.restype = i32
         L.fpx_debug_last_tally_path.argtypes = [vp]; L.fpx_debug_last_tally_path.restype = i32

@@ -23,6 +23,7 @@
 #include "fpx_depgraph.cuh"
 #include "fpx_epaxos.cuh"
 #include "fpx_ranges.cuh"
+#include "fpx_reads.cuh"
 #include "fpx_replica_misc.cuh"
 #include "fpx_tally.cuh"
 #include "fpx_vanilla.cuh"
@@ -1244,3 +1245,4 @@ int fpx_snapshot_log(fpx_engine* e, int32_t first_slot, int32_t n_slots, int32_t
 
 #include "fpx_engine_epaxos.inc"
 #include "fpx_engine_f4.inc"
+#include "fpx_engine_reads.inc"

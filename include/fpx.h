@@ -661,6 +661,91 @@ int fpx_global_watermark(fpx_engine* e, uint32_t epoch, int32_t timeout_ms, int3
  * not vacant); a client request is ignored (the reference's check(!log.contains) drops a duplicate). */
 int fpx_retire_below(fpx_engine* e, int32_t slot);
 
+/* ---- MultiPaxos linearizable reads (S/multipaxos/MultiPaxos.proto:36-115) ---------------------------------
+ * A read learns a slot from a read quorum of acceptors, then a replica answers it once its log has executed
+ * that slot.  One fpx_reads handle holds one of the two read-quorum tallies (the Client's or a ReadBatcher's)
+ * and one replica's deferred reads, on the device, stream and quorum geometry of a FPX_MULTIPAXOS engine.  Once
+ * that engine is destroyed, fpx_reads_destroy is the only call the handle takes.
+ *
+ * The acceptor side needs no entry point.  Acceptor.handleMaxSlotRequest / handleBatchMaxSlotRequest
+ * (S/multipaxos/Acceptor.scala:222-254) answer {groupIndex, index, maxVotedSlot}; a MaxSlotRequest is a batch
+ * boundary of its acceptor's Phase2a stream, and fpx_snapshot_acceptor(..., n_slots = 0) at that boundary
+ * returns the maxVotedSlot every request queued there is answered with.
+ * Not reproduced: the unsafeReadAtI and unsafeReadAtFirstSlot options (Client.scala:892-898), the
+ * state-machine execution of a read (the caller runs the read right after log entry after_slot), and the
+ * ReadReplyBatch fan-out to a ProxyReplica (Replica.scala:369-390); all stay with the caller.
+ *
+ * kind FPX_READS_CLIENT: Client.handleMaxSlotReply (S/multipaxos/Client.scala:851-931).  Replies are keyed
+ *   by (group, acceptor) (:877-879); the read completes at f+1 replies (:880), flexible: on Grid.isReadQuorum
+ *   (:883-887); slot = max + numAcceptorGroups - 1, flexible: max (:892-898).
+ * kind FPX_READS_READ_BATCHER: ReadBatcher.handleBatchMaxSlotReply (S/multipaxos/ReadBatcher.scala:568-623).
+ *   Replies are keyed by acceptorIndex only, the group is ignored (:584); the read completes at f+1 replies
+ *   even on a flexible config (:585); slot = max + numAcceptorGroups - 1 (:592-598, acceptors :207-211); the
+ *   entry is removed on completion (:601).
+ * A read is (key, id): key < key_capacity is the caller's handle for a Client pseudonym or a ReadBatcher id
+ * slot, id the generation (clientId / readBatcherId).  Memory: key_capacity x (32 + 8 x voters) bytes,
+ * voters = numAcceptorGroups x acceptors_per_group (Client) or acceptors_per_group (ReadBatcher). */
+typedef struct fpx_reads fpx_reads;
+enum { FPX_READS_CLIENT = 0, FPX_READS_READ_BATCHER = 1 };
+typedef struct { int32_t key, id; } fpx_read_open;
+/* MaxSlotReply / BatchMaxSlotReply (MultiPaxos.proto) with the read's key; voter = group<<16 | acceptor */
+typedef struct { int32_t key, id, voter, slot; } fpx_max_slot_reply;
+/* a completed read: the slot its ReadRequest carries */
+typedef struct { int32_t key, id, slot, reserved; } fpx_read_slot;
+/* ReadRequest / SequentialReadRequest {slot}; a *Batch form is one record per command with the batch's slot;
+ * EventualReadRequest is slot = -1.  handle is the caller's id of the read. */
+typedef struct { int32_t slot, handle; } fpx_read_request;
+/* ReadReply.slot = reply_slot; after_slot = the last log entry executed before the read runs */
+typedef struct { int32_t handle, reply_slot, after_slot, reserved; } fpx_read_reply;
+
+int fpx_reads_create(fpx_reads** out, fpx_engine* e, int32_t kind, int32_t key_capacity, int32_t pending_capacity,
+                     int32_t max_batch);
+void fpx_reads_destroy(fpx_reads* r);
+/* Client.readImpl (Client.scala:626-660): states(pseudonym) = MaxSlot(id, {}); ReadBatcher (ReadBatcher.scala:472):
+ * batchMaxSlotReplies(id) = Map().  Opening an open key again replaces its read; the last record of a key in
+ * the batch wins.  key outside [0, key_capacity): FPX_ERR_INVALID_ARG with its index, nothing applied. */
+int fpx_reads_open(fpx_reads* r, const fpx_read_open* in, int32_t n, int64_t* err_index);
+/* The tally of the handle's kind, replies in delivery order.  A reply whose key is not open, whose read is
+ * complete, or whose id differs is ignored (Client.scala:858-874, ReadBatcher.scala:572-580), and so is a key
+ * outside [0, key_capacity).  A second reply of a voter overwrites its first; the slot is the maximum over the
+ * latest reply of each voter at the completing reply; slot arithmetic wraps like a JVM Int.  out receives
+ * one record per read completed in the batch, ORDERED BY THE INDEX OF THE COMPLETING REPLY; capacity n.
+ * A counted reply whose voter is no acceptor of the config is FPX_ERR_BAD_ACCEPTOR at its index: with the
+ * flexible Client this is Grid.isReadQuorum's `require` (S/quorums/Grid.scala:36-39), elsewhere such a reply
+ * cannot arrive.  The handle's read state after an error is unspecified, as the reference's actor has failed. */
+int fpx_reads_max_slot_replies(fpx_reads* r, const fpx_max_slot_reply* in, int32_t n, fpx_read_slot* out,
+                               int32_t* n_out, int64_t* err_index);
+/* Replica.handleReadRequest / handleSequentialReadRequest / handleEventualReadRequest and their *Batch forms
+ * (Replica.scala:629-689) -> handleDeferrableRead(s) (:463-529) against the handle's executed watermark W
+ * (0 at creation).  slot < W: answered now, in delivery order, reply {handle, W - 1, W - 1, 0} (:521-527);
+ * any other read waits in the pending pool (:468-478).  out receives the immediate replies; capacity n.
+ * More pending reads than pending_capacity: FPX_ERR_OVERFLOW_FULL at the first deferred read that does not
+ * fit, and nothing of the batch is applied (n_out = 0). */
+int fpx_reads_replica(fpx_reads* r, const fpx_read_request* in, int32_t n, fpx_read_reply* out, int32_t* n_out,
+                      int64_t* err_index);
+/* executeLog (Replica.scala:394-413) up to watermark: W = watermark, and every pending read with slot < W
+ * leaves, by slot and by arrival within a slot, as {handle, slot - 1, slot, 0}: it runs right after log entry
+ * `slot`, and its ReadReply.slot is slot - 1 because processDeferredReads runs before executedWatermark += 1
+ * (:405-413) -- a quirk of the reference, kept.  watermark < W: FPX_ERR_INVALID_ARG.  W is
+ * fpx_chosen_watermark with one shard, fpx_global_watermark with several.  out capacity pending_capacity. */
+int fpx_reads_advance(fpx_reads* r, int32_t watermark, fpx_read_reply* out, int32_t* n_out);
+/* The same on DEVICE pointers, asynchronous on the engine's stream (fpx_stream); the status, the first
+ * offending index and the output counts are collected by fpx_reads_sync.  fpx_reads_advance_dev reads the
+ * watermark from d_watermark on the device, e.g. the one fpx_step_dev writes: no host round trip. */
+int fpx_reads_max_slot_replies_dev(fpx_reads* r, const fpx_max_slot_reply* d_in, int32_t n, fpx_read_slot* d_out);
+int fpx_reads_replica_dev(fpx_reads* r, const fpx_read_request* d_in, int32_t n, fpx_read_reply* d_out);
+int fpx_reads_advance_dev(fpx_reads* r, const int32_t* d_watermark, fpx_read_reply* d_out);
+typedef struct {
+  int32_t status;       /* first (lowest record index) error of any call since the last sync */
+  int32_t watermark;    /* the handle's W                                                     */
+  int64_t err_index;
+  int32_t n_slots;      /* of the last fpx_reads_max_slot_replies_dev                         */
+  int32_t n_replies;    /* of the last fpx_reads_replica_dev                                  */
+  int32_t n_released;   /* of the last fpx_reads_advance_dev                                  */
+  int32_t n_pending;    /* reads waiting in the pool                                          */
+} fpx_reads_sync_result;
+int fpx_reads_sync(fpx_reads* r, fpx_reads_sync_result* out);
+
 /* The engine's CUDA stream (a cudaStream_t) so a caller can order its own work
  * (events, NCCL collectives) with the engine's. */
 void* fpx_stream(fpx_engine* e);
