@@ -34,6 +34,9 @@ using namespace fpx;
 constexpr int kMaxEvents = 16;
 constexpr int kTallySmem = 200 * 1024 / (1024 / kTT);  // dynamic shared memory of a tally CTA (one CTA of 1024 threads per SM)
 constexpr int kStepRing = 1024;
+// votes one tally launch takes: its scan of the per-chunk counts (4 B per 1024 votes) uses at most 40 KB of the
+// dynamic shared memory; a larger call is cut into several launches (tally_launch)
+constexpr int32_t kTallyMaxSub = (40 * 1024 / 4) * kChunkVotes;
 
 struct fpx_engine {
   fpx_config cfg;
@@ -338,7 +341,7 @@ int fpx_create(fpx_engine** out, const fpx_config* cfg) {
     // the tally's dynamic shared memory: scan of the per-chunk counts (4 B per 1024 votes) + the CTA's kept
     // {vote, value} entries of the sweep (8 B per window row); one launch takes at most 40 KB of it for the scan
     const int smem_cap = kTallySmem;
-    e->tally_max_sub = (40 * 1024 / 4) * kChunkVotes;
+    e->tally_max_sub = kTallyMaxSub;
     const void* tk = tally_kernel_ptr(g.row_words);
     CKC(cudaFuncSetAttribute(tk, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_cap));
     CKC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, tk, kTT, smem_cap));
@@ -496,6 +499,13 @@ int fpx_debug_set_acceptor_segments(fpx_engine* e, int32_t segments) {
   e->acc_segments = segments;
   return FPX_OK;
 }
+// Undocumented test aid: cut every tally call into launches of at most `votes` votes (1 .. kTallyMaxSub;
+// 0 = kTallyMaxSub), so that small batches run the state a call carries from one launch to the next.
+int fpx_debug_set_tally_max_sub(fpx_engine* e, int32_t votes) {
+  if (!e || votes < 0 || votes > kTallyMaxSub) return FPX_ERR_INVALID_ARG;
+  e->tally_max_sub = votes == 0 ? kTallyMaxSub : votes;
+  return FPX_OK;
+}
 int fpx_debug_last_tally_path(fpx_engine* e) {
   if (!e) return FPX_ERR_INVALID_ARG;
   uint32_t v = 0;
@@ -628,6 +638,7 @@ static int tally_launch(fpx_engine* e, const fpx_p2b* d_in, int32_t n, fpx_chose
     P.cc = e->t_cc;
     P.tmp = (int2*)e->t_tmp;
     P.first = done == 0;
+    P.index_base = done;                           // error indices are call indices (first offender in delivery order)
     P.path = e->tally_path;
     P.votes = e->votes;
     P.rlog = fuse ? e->rlog : nullptr;

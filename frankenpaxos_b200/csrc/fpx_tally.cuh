@@ -67,6 +67,7 @@ struct TallyParams {
   uint32_t* cc;            // [ceil(n/1024)]    completing votes per 1024-vote chunk
   int2* tmp;               // [n] exact path: Chosen record of completing vote i, parked at i
   int32_t first;           // 1: output offset 0, else append at st->n_chosen (sub-launches of one call)
+  int32_t index_base;      // call index of in[0]: error indices count from the call's first vote, not the launch's
   int32_t path;            // 0: sweep when sound; 2: always the exact per-vote path (tests, A/B); 4: profiling, no REDs
   int32_t keep_cap;        // rows of the window one CTA can keep in shared memory between phases B and D
   unsigned long long* votes;  // vanilla Mencius: the coordinator's log entry turns ChosenEntry on completion
@@ -294,7 +295,7 @@ __device__ __forceinline__ void tally_exact(const TallyParams& P, int wlo, int w
           // several rounds of this slot were armed: the key lives in the table
           RowRef rr = find_row(g, P.pl, local_slot(g, rec[u].z), rec[u].z, rec[u].w);
           if (rr.p == nullptr) {
-            if (!kRedo) report_error(P.st, FPX_ERR_UNKNOWN_SLOT_ROUND, i);            // :220-225
+            if (!kRedo) report_error(P.st, FPX_ERR_UNKNOWN_SLOT_ROUND, (long long)P.index_base + i);   // :220-225
             ok = false;
           } else if (!kRedo) {
             const int v = voter_index(g, rec[u].x, rec[u].y, rec[u].z);
@@ -307,7 +308,7 @@ __device__ __forceinline__ void tally_exact(const TallyParams& P, int wlo, int w
           }
         } else if (hw == kUnarmed || (int)hw != rec[u].w) {
           // the slot has one armed round and it is not this vote's: never armed (:220-225)
-          report_error(P.st, FPX_ERR_UNKNOWN_SLOT_ROUND, i);
+          report_error(P.st, FPX_ERR_UNKNOWN_SLOT_ROUND, (long long)P.index_base + i);
           ok = false;
         }
         if (ok) {
@@ -320,7 +321,7 @@ __device__ __forceinline__ void tally_exact(const TallyParams& P, int wlo, int w
             const int v = voter_index(g, rec[u].x, rec[u].y, rec[u].z);
             if (v < 0) {
               // Grid.isWriteQuorum `require(xs subsetOf nodes)` (Grid.scala:44-47)
-              report_error(P.st, FPX_ERR_BAD_ACCEPTOR, i);
+              report_error(P.st, FPX_ERR_BAD_ACCEPTOR, (long long)P.index_base + i);
             } else {
               uint32_t mine = 0;
 #pragma unroll
@@ -369,7 +370,7 @@ __device__ __forceinline__ void tally_stamp_checked(const TallyParams& P, int wl
         if (i < whi) {
           int local = local_slot(g, rec[u].z);
           if (local < 0) {
-            if (local != kLocalRetired) report_error(P.st, FPX_ERR_SLOT_RANGE, i);
+            if (local != kLocalRetired) report_error(P.st, FPX_ERR_SLOT_RANGE, (long long)P.index_base + i);
           } else {
             row[u] = P.pl.rows + (size_t)local * g.row_words;
             rw[u] = __ldcg(row[u]);
@@ -384,7 +385,7 @@ __device__ __forceinline__ void tally_stamp_checked(const TallyParams& P, int wl
         // Server.handlePhase2b: no Phase 2 for the slot / already chosen -> ignore
         // (:1088-1106); stale round -> ignore (:1109-1112); a larger round fails checkEq (:1116)
         if (w == kUnarmed || (w & kDoneBit) || rec[u].w < (int)w) continue;
-        if (rec[u].w > (int)w) { report_error(P.st, FPX_ERR_UNKNOWN_SLOT_ROUND, i); continue; }
+        if (rec[u].w > (int)w) { report_error(P.st, FPX_ERR_UNKNOWN_SLOT_ROUND, (long long)P.index_base + i); continue; }
         int v = voter_index(g, rec[u].x, rec[u].y, rec[u].z);
         if (v < 0) continue;
         red_min_u32(&row[u][2 + v], P.seq_base + (uint32_t)i);
@@ -449,7 +450,7 @@ __global__ void __launch_bounds__(kTT, 1024 / kTT) tally_kernel(TallyParams P) {
         if (i >= whi) continue;
         int local = local_slot(g, rec[u].z);
         if (local < 0) {   // a retired slot was chosen long ago: the vote finds `Done` (:227-232)
-          if (local != kLocalRetired) report_error(P.st, FPX_ERR_SLOT_RANGE, i);
+          if (local != kLocalRetired) report_error(P.st, FPX_ERR_SLOT_RANGE, (long long)P.index_base + i);
           continue;
         }
         const int rel = ring_to_rel(g, local);

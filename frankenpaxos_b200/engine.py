@@ -156,6 +156,10 @@ class Engine:
         """Cut every acceptor launch into `segments` pipelined segments (0: automatic, from the L2 size)."""
         self._check(self._L.fpx_debug_set_acceptor_segments(self.h, segments))
 
+    def set_tally_max_sub(self, votes):
+        """Cut every tally call into launches of at most `votes` votes (0: the default, 10,485,760)."""
+        self._check(self._L.fpx_debug_set_tally_max_sub(self.h, votes))
+
     @property
     def last_tally_path(self):
         """'sweep' / 'exact': what the last proxyleader_phase2b launch did."""

@@ -35,9 +35,12 @@ def row_words(cfg):
     return 8 if v <= 6 else (16 if v <= 14 else 32)
 
 
-def make_pair(cfg, slot_capacity, max_batch=1 << 16, overflow_capacity=1 << 8, **kw):
+def make_pair(cfg, slot_capacity, max_batch=1 << 16, overflow_capacity=1 << 8, tally_max_sub=0, **kw):
+    """tally_max_sub > 0: the engine cuts every tally call into launches of at most that many votes."""
     eng = Engine(slot_capacity=slot_capacity, max_batch=max_batch, overflow_capacity=overflow_capacity,
                  **cfg, **kw)
+    if tally_max_sub:
+        eng.set_tally_max_sub(tally_max_sub)
     ora = O.MultiPaxos(cfg["f"], cfg["num_acceptor_groups"], cfg["acceptors_per_group"],
                        cfg.get("flexible", False), cfg.get("num_leaders"), cfg.get("num_replicas"))
     return eng, ora
@@ -112,12 +115,13 @@ def compare_log(eng, ora, first_slot, n_slots):
     same(eng.snapshot_log(first_slot, n_slots), ora.snapshot_log(first_slot, n_slots), "replica log")
 
 
-def adversarial(cfg, seed, n_slots, kmax, coop_ctas_per_sm=0, max_batch=1 << 16):
+def adversarial(cfg, seed, n_slots, kmax, coop_ctas_per_sm=0, max_batch=1 << 16, tally_max_sub=0):
     """Random rounds (stale and fresh), duplicate deliveries, late votes, several live rounds per slot (so
     armed rows move to the overflow table), non-thrifty fan-out, many small and large batches; every
     acceptor and the replica log compared after each phase."""
     g = T.rng(seed)
-    eng, ora = make_pair(cfg, n_slots, max_batch=max_batch, overflow_capacity=1 << 13 if n_slots <= 3000 else 1 << 20)
+    eng, ora = make_pair(cfg, n_slots, max_batch=max_batch, overflow_capacity=1 << 13 if n_slots <= 3000 else 1 << 20,
+                         tally_max_sub=tally_max_sub)
     eng.set_coop_ctas_per_sm(coop_ctas_per_sm)
     for phase in range(4):
         k = int(g.integers(1, kmax))

@@ -613,7 +613,8 @@ def test_phase1a_and_safe_values(shape):
 def test_full_size_properties_cfg3():
     """BASELINE cfg3 at full size: 2x3 grid, 2^22 slots, thrifty write quorum = one grid
     column (2 votes per slot), 10 proxy-leader partitions (slot % 10) shuffled within a
-    partition; 8.4M-record batches (two tally launches).  Size-independent properties."""
+    partition; 8.4M-record batches (one tally launch: the split starts above 10,485,760 votes, see
+    test_tally_split_gpu.py).  Size-independent properties."""
     cfg, n_slots = T.config_by_name("cfg3")
     eng = Engine(slot_capacity=n_slots, max_batch=2 * n_slots, **cfg)
     a, p, b = T.workload(1, cfg, n_slots, partitions=10)
