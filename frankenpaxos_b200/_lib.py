@@ -32,6 +32,9 @@ SYMBOLS = [
     "fpx_epaxos_preacceptok_dev", "fpx_epaxos_acceptok_dev", "fpx_epaxos_preaccept_sets",
     "fpx_epaxos_create", "fpx_epaxos_destroy", "fpx_epaxos_lead", "fpx_epaxos_preaccept", "fpx_epaxos_accept",
     "fpx_epaxos_preacceptok", "fpx_epaxos_acceptok", "fpx_epaxos_entry", "fpx_epaxos_last_kernel_ms", "fpx_depset_union", "fpx_depset_union_dense_dev",
+    "fpx_epaxos_commit", "fpx_epaxos_nack", "fpx_epaxos_prepare_phase", "fpx_epaxos_prepare", "fpx_epaxos_prepareok",
+    "fpx_epaxos_slow_path_timer", "fpx_epaxos_commit_dev", "fpx_epaxos_nack_dev", "fpx_epaxos_prepare_phase_dev",
+    "fpx_epaxos_prepare_dev", "fpx_epaxos_prepareok_dev", "fpx_epaxos_slow_path_timer_dev",
     "fpx_reads_create", "fpx_reads_destroy", "fpx_reads_open", "fpx_reads_max_slot_replies", "fpx_reads_replica",
     "fpx_reads_advance", "fpx_reads_max_slot_replies_dev", "fpx_reads_replica_dev", "fpx_reads_advance_dev", "fpx_reads_sync",
 ]

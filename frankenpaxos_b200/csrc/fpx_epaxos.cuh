@@ -31,12 +31,19 @@ enum { EK_NONE = 0, EK_NOCOMMAND = 1, EK_PREACCEPTED = 2, EK_ACCEPTED = 3, EK_CO
 // leader row words: header | accept-phase deps | AcceptOk stamps | PreAcceptOk stamps | one 32-byte answer
 // {seq, deps[7]} per replica.  A response touches the header sector, one stamp word and one answer sector;
 // counting a quorum reads one stamp sector.
+// A Preparing row (transitionToPreparePhase, :969-996) keeps its ballot in L_BORD / L_BREP, its PrepareOk
+// first-delivery stamps in L_RSTAMP and replica k's PrepareOk {vb_ord, vb_rep, status, value} in sector k of L_RESP.
 enum { L_KIND = 0, L_VALUE, L_BORD, L_BREP, L_FLAGS, L_ASEQ, L_PAD0, L_PAD1, L_ADEPS = 8, L_ASTAMP = 16, L_RSTAMP = 24, L_RESP = 32 };
-enum { LK_NONE = 0, LK_PREACCEPTING = 1, LK_ACCEPTING = 2 };
+enum { LK_NONE = 0, LK_PREACCEPTING = 1, LK_ACCEPTING = 2, LK_PREPARING = 3 };
 constexpr int kEpRespWords = 8;     // {seq, deps[7]} (n <= 7)
 enum { LF_AVOID = 1, LF_TIMER = 2 };
 enum { REPLY_NONE = 0, REPLY_OK = 1, REPLY_NACK = 2, REPLY_COMMIT = 3 };
 enum { EV_NONE = 0, EV_FAST_COMMIT = 1, EV_SLOW_ACCEPT = 2, EV_TIMER = 3, EV_COMMIT = 4 };
+enum { EV_RECOVER_TIMER = 1 };                                   // Nack outcome
+enum { EV_RESTART = 1 };                                         // PrepareOk outcome
+enum { ST_NOT_SEEN = 0, ST_PRE_ACCEPTED = 1, ST_ACCEPTED = 2 };  // CommandStatus (EPaxos.proto:91-95)
+// response kinds of the stamp / decide passes
+enum { kRespPreAcceptOk = 0, kRespAcceptOk = 1, kRespPrepareOk = 2 };
 
 struct EpGeometry {
   int32_t f, n, index, fast_quorum, slow_quorum;
@@ -315,7 +322,10 @@ __global__ void __launch_bounds__(kEpTile) ep_acceptor_kernel(EpParams P) {
 
 // Nack(instance, largestBallot) carries largestBallot AS OF that delivery (:1166-1167): the max over the
 // handle's value at batch start and the ballots of the records that proceeded before it -- an exclusive
-// prefix max over the batch.  Three small passes, run only when the batch produced a Nack.
+// prefix max over the batch.  Three small passes, run only when the batch produced a Nack.  handlePrepare
+// raises largestBallot before it builds its Nack (:1637, :1652): there every record contributes and the max is
+// inclusive, floored at (0, index) (the reference's initial largestBallot, :458); the ballot goes to columns
+// col, col+1 of the reply row.
 constexpr int kEpScanTile = 1024;
 __global__ void __launch_bounds__(kEpScanTile) ep_nack_tilemax_kernel(EpParams P, unsigned long long* tile_max) {
   if (!(__ldcg(&P.s.st->ts_flags) & 1u)) return;
@@ -331,13 +341,14 @@ __global__ void __launch_bounds__(kEpScanTile) ep_nack_tilemax_kernel(EpParams P
     tile_max[blockIdx.x] = m;
   }
 }
-__global__ void __launch_bounds__(kEpScanTile) ep_nack_fixup_kernel(EpParams P, int WO, const unsigned long long* tile_max) {
+__global__ void __launch_bounds__(kEpScanTile) ep_nack_fixup_kernel(EpParams P, int WO, const unsigned long long* tile_max,
+                                                                    int col, bool inclusive, unsigned long long floor) {
   if (!(__ldcg(&P.s.st->ts_flags) & 1u)) return;
   __shared__ unsigned long long s_w[32];
   __shared__ unsigned long long s_carry;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   // carry into this tile: largestBallot at batch start and every earlier tile
-  unsigned long long c = tid == 0 ? P.s.largest[0] : 0ull;
+  unsigned long long c = tid == 0 ? max(P.s.largest[0], floor) : 0ull;
   for (int t = tid; t < (int)blockIdx.x; t += kEpScanTile) c = max(c, tile_max[t]);
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) c = max(c, __shfl_xor_sync(0xffffffffu, c, d));
@@ -360,13 +371,13 @@ __global__ void __launch_bounds__(kEpScanTile) ep_nack_fixup_kernel(EpParams P, 
   for (int w = 0; w < warp; ++w) pre = max(pre, s_w[w]);
   unsigned long long excl = __shfl_up_sync(0xffffffffu, incl, 1);
   if (lane == 0) excl = 0;
-  excl = max(excl, pre);
+  excl = max(inclusive ? incl : excl, pre);
   if (i < P.n_rec) {
     int32_t* o = P.out + (size_t)i * WO;
     if (o[0] == REPLY_NACK) {
       int ord, rep;
       key_ballot(excl, ord, rep);
-      o[1] = ord; o[2] = rep;
+      o[col] = ord; o[col + 1] = rep;
     }
   }
 }
@@ -403,18 +414,33 @@ __device__ __forceinline__ void ep_store8(int32_t* p, const int (&v)[8]) {
   __stcg((int4*)p, make_int4(v[0], v[1], v[2], v[3]));
   __stcg((int4*)p + 1, make_int4(v[4], v[5], v[6], v[7]));
 }
-// the answer {seq, deps[n], 0...} carried by PreAcceptOk row r
+// the answer {seq, deps[n], 0...} carried by PreAcceptOk row r; {vb_ord, vb_rep, status, value, 0...} by
+// PrepareOk row r
+template <int kWhich>
 __device__ __forceinline__ void ep_answer_of(const EpGeometry& g, const int32_t* r, int (&v)[8]) {
+  if (kWhich == kRespPrepareOk) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) v[k] = k < 4 ? r[5 + k] : 0;
+    return;
+  }
   v[0] = r[5];
 #pragma unroll
   for (int k = 0; k < 7; ++k) v[1 + k] = k < g.n ? r[6 + k] : 0;
 }
+// in-row words of the response handlers: PreAcceptOk 6+n, AcceptOk 6, PrepareOk 9
+template <int kWhich>
+__host__ __device__ __forceinline__ int ep_resp_in_words(const EpGeometry& g) {
+  return kWhich == kRespAcceptOk ? 6 : kWhich == kRespPrepareOk ? 9 : 6 + g.n;
+}
 
-template <bool kAccept>
+// the leader kinds the three response handlers count for: PreAcceptOk (:1295-1315), AcceptOk (:1518-1535),
+// PrepareOk (:1763-1784)
+template <int kWhich>
 __global__ void __launch_bounds__(kEpTile) ep_response_stamp_kernel(EpParams P, int32_t* mode) {
+  constexpr bool kAccept = kWhich == kRespAcceptOk, kPrepare = kWhich == kRespPrepareOk;
   const EpGeometry& g = P.g;
   extern __shared__ int32_t s_ep[];
-  const int W = kAccept ? 6 : 6 + g.n, Wp = W | 1;
+  const int W = ep_resp_in_words<kWhich>(g), Wp = W | 1;
   const int tid = threadIdx.x;
   const long long tile0 = (long long)blockIdx.x * kEpTile;
   const int rows = (int)min((long long)kEpTile, P.n_rec - tile0);
@@ -430,23 +456,25 @@ __global__ void __launch_bounds__(kEpTile) ep_response_stamp_kernel(EpParams P, 
   } else {
     int32_t* l = P.s.lead + inst * kEpLeadWords;
     const int4 h = __ldcg((const int4*)l);                                      // {kind, value, bord, brep}
-    if (h.x == (kAccept ? LK_ACCEPTING : LK_PREACCEPTING) &&                    // :1295-1315 / :1518-1535
-        ballot_key(r[2], r[3]) == ballot_key(h.z, h.w)) {                       // :1325-1335 / :1543-1552
+    const bool leading = h.x == (kAccept ? LK_ACCEPTING : kPrepare ? LK_PREPARING : LK_PREACCEPTING);
+    if (kPrepare && leading && ballot_key(r[2], r[3]) > ballot_key(h.z, h.w))
+      report_error(P.s.st, FPX_ERR_CHECK_FAILED, i);                            // logger.checkLt (:1792)
+    if (leading && ballot_key(r[2], r[3]) == ballot_key(h.z, h.w)) {            // :1325-1335 / :1543-1552 / :1785
       ep_count(P.s, inst, P.tag);
       const uint32_t seq = P.seq_base + (uint32_t)i;
       const uint32_t old = atomicMin((uint32_t*)&l[(kAccept ? L_ASTAMP : L_RSTAMP) + r[4]], seq);
-      if (old == kStampEmpty) {                                 // responses(replicaIndex) = ok (:1340), new key
+      if (old == kStampEmpty) {                                 // responses(replicaIndex) = ok (:1340 / :1796), new key
         md = 1;
         if (!kAccept) {
           int v[8];
-          ep_answer_of(g, r, v);
+          ep_answer_of<kWhich>(g, r, v);
           ep_store8(l + L_RESP + r[4] * kEpRespWords, v);
         }
       } else if (old >= P.seq_base) {                           // two responses of one replica in one batch (E2)
         report_error(P.s.st, FPX_ERR_BATCH_ORDER, max((uint32_t)i, old - P.seq_base));
       } else if (!kAccept) {
         int v[8], have[8];
-        ep_answer_of(g, r, v);
+        ep_answer_of<kWhich>(g, r, v);
         ep_load8(l + L_RESP + r[4] * kEpRespWords, have);
         bool same = true;
 #pragma unroll
@@ -458,14 +486,73 @@ __global__ void __launch_bounds__(kEpTile) ep_response_stamp_kernel(EpParams P, 
   mode[i] = md;
 }
 
-// decide pass: events at the first crossing of the quorum thresholds.  out row: {event, seq, deps[n]}, staged
-// in shared memory and stored coalesced.
-template <bool kAccept>
+// preAcceptingSlowPath (:796-813) over the answers in[a] of leader row l, then transitionToAcceptPhase
+// (:732-793): event {EV_SLOW_ACCEPT, seq, deps[n]} into o, cmdLog row c Accepted, l Accepting with only the
+// leader's own AcceptOk.  h0 = the leader header {kind, value, bord, brep}.
+__device__ __forceinline__ void ep_slow_path(const EpGeometry& g, int32_t* l, int32_t* c, const int4& h0,
+                                             const int (&ans)[kEpMaxN - 1][8], const bool (&in)[kEpMaxN - 1], int32_t* o) {
+  int sseq = INT_MIN;
+  int sdeps[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+#pragma unroll
+  for (int a = 0; a < kEpMaxN - 1; ++a) {
+    if (!in[a]) continue;
+    sseq = max(sseq, ans[a][0]);
+#pragma unroll
+    for (int k = 0; k < 7; ++k) if (k < g.n) sdeps[k] = max(sdeps[k], ans[a][1 + k]);   // dependencies.addAll (:804-807)
+  }
+  o[0] = EV_SLOW_ACCEPT; o[1] = sseq;
+#pragma unroll
+  for (int k = 0; k < 7; ++k) if (k < g.n) o[2 + k] = sdeps[k];
+  // transitionToAcceptPhase (:732-793)
+  __stcg((int4*)c, make_int4(EK_ACCEPTED, h0.y, h0.z, h0.w));
+  __stcg((int4*)c + 1, make_int4(h0.z, h0.w, sseq, 0));
+  ep_store8(c + C_DEPS, sdeps);
+  l[L_ASEQ] = sseq;
+  ep_store8(l + L_ADEPS, sdeps);
+  int as[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) as[k] = k == g.index ? 0 : (int)kStampEmpty;   // own AcceptOk (:781-789)
+  ep_store8(l + L_ASTAMP, as);
+  l[L_KIND] = LK_ACCEPTING;
+}
+
+// out-row words of the response handlers: events {kind, seq, deps[n]}, PrepareOk {kind, b_ord, b_rep, value}
+template <int kWhich>
+__host__ __device__ __forceinline__ int ep_resp_out_words(const EpGeometry& g) {
+  return kWhich == kRespPrepareOk ? 4 : 2 + g.n;
+}
+
+// handlePrepareOk's decision (:1804-1867) over the PrepareOks in[a] {vb_ord, vb_rep, status, value}: the
+// maximum vote ballot, then the first PreAccepted response of that ballot -- lowest replica index first --
+// or Noop.  The two branches before it cannot be taken in the reference and are not taken here: the
+// `status == Some(Accepted)` test (:1813) compares an enum with an Option, and the fast-path candidates
+// (:1836) require p.ballot == Ballot(0, _) while p.ballot is the Preparing ballot, of ordering >= 1.
+__device__ __forceinline__ int ep_prepare_decide(const EpGeometry& g, const int (&ans)[kEpMaxN - 1][8],
+                                                 const bool (&in)[kEpMaxN - 1]) {
+  unsigned long long vmax = 0;
+#pragma unroll
+  for (int a = 0; a < kEpMaxN - 1; ++a)
+    if (in[a]) vmax = max(vmax, ballot_key(ans[a][0], ans[a][1]));
+  int value = FPX_VALUE_NOOP;
+  bool found = false;
+#pragma unroll
+  for (int a = 0; a < kEpMaxN - 1; ++a) {
+    if (found || !in[a] || ballot_key(ans[a][0], ans[a][1]) != vmax || ans[a][2] != ST_PRE_ACCEPTED) continue;
+    value = ans[a][3];
+    found = true;
+  }
+  return value;
+}
+
+// decide pass: events at the first crossing of the quorum thresholds.  out row: {event, seq, deps[n]} (PrepareOk:
+// {kind, b_ord, b_rep, value}), staged in shared memory and stored coalesced.
+template <int kWhich>
 __global__ void __launch_bounds__(kEpTile) ep_response_decide_kernel(EpParams P, const int32_t* mode) {
+  constexpr bool kAccept = kWhich == kRespAcceptOk, kPrepare = kWhich == kRespPrepareOk;
   const EpGeometry& g = P.g;
   extern __shared__ int32_t s_ep[];
-  const int W = kAccept ? 6 : 6 + g.n, Wp = W | 1;
-  const int WO = 2 + g.n;                                       // odd: conflict-free as it is
+  const int W = ep_resp_in_words<kWhich>(g), Wp = W | 1;
+  const int WO = ep_resp_out_words<kWhich>(g);                  // odd for events: conflict-free as it is
   int32_t* s_out = s_ep + kEpTile * Wp;
   const int tid = threadIdx.x;
   const long long tile0 = (long long)blockIdx.x * kEpTile;
@@ -491,7 +578,7 @@ __global__ void __launch_bounds__(kEpTile) ep_response_decide_kernel(EpParams P,
           report_error(P.s.st, FPX_ERR_BATCH_ORDER, i);
         } else {
           int v[8];
-          ep_answer_of(g, r, v);
+          ep_answer_of<kWhich>(g, r, v);
           ep_store8(l + L_RESP + r[4] * kEpRespWords, v);
         }
       } else {
@@ -502,7 +589,21 @@ __global__ void __launch_bounds__(kEpTile) ep_response_decide_kernel(EpParams P,
         for (int k = 0; k < 8; ++k) before += (k < g.n && (uint32_t)st[k] < seq);
         const int after = before + 1;
         const int4 h0 = __ldcg((const int4*)l);                 // {kind, value, bord, brep}
-        if (kAccept) {
+        if (kPrepare) {
+          if (before < g.slow_quorum && after >= g.slow_quorum) {                 // :1800-1802
+            int ans[kEpMaxN - 1][8];
+            bool in[kEpMaxN - 1];
+#pragma unroll
+            for (int a = 0; a < kEpMaxN - 1; ++a) {
+              in[a] = a < g.n && (uint32_t)st[a] <= seq;
+              if (in[a]) ep_load8(l + L_RESP + a * kEpRespWords, ans[a]);
+            }
+            // transitionToPreAcceptPhase(instance, ballot, value, avoidFastPath = true) (:1856-1867) is the
+            // caller's fpx_epaxos_lead; until then the row leads nothing
+            o[0] = EV_RESTART; o[1] = h0.z; o[2] = h0.w; o[3] = ep_prepare_decide(g, ans, in);
+            l[L_KIND] = LK_NONE;
+          }
+        } else if (kAccept) {
           if (before < g.slow_quorum && after >= g.slow_quorum) {                 // :1558-1560
             int ad[8];
             ep_load8(l + L_ADEPS, ad);
@@ -568,29 +669,7 @@ __global__ void __launch_bounds__(kEpTile) ep_response_decide_kernel(EpParams P,
               ep_store8(c + C_DEPS, fdeps);
               l[L_KIND] = LK_NONE;
             } else if (slow) {                                                   // preAcceptingSlowPath :796-813
-              int sseq = INT_MIN;
-              int sdeps[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-#pragma unroll
-              for (int a = 0; a < kEpMaxN - 1; ++a) {
-                if (!in[a]) continue;
-                sseq = max(sseq, ans[a][0]);
-#pragma unroll
-                for (int k = 0; k < 7; ++k) if (k < g.n) sdeps[k] = max(sdeps[k], ans[a][1 + k]);   // dependencies.addAll (:804-807)
-              }
-              o[0] = EV_SLOW_ACCEPT; o[1] = sseq;
-              #pragma unroll
-              for (int k = 0; k < 7; ++k) if (k < g.n) o[2 + k] = sdeps[k];
-              // transitionToAcceptPhase (:732-793)
-              __stcg((int4*)c, make_int4(EK_ACCEPTED, h0.y, h0.z, h0.w));
-              __stcg((int4*)c + 1, make_int4(h0.z, h0.w, sseq, 0));
-              ep_store8(c + C_DEPS, sdeps);
-              l[L_ASEQ] = sseq;
-              ep_store8(l + L_ADEPS, sdeps);
-              int as[8];
-#pragma unroll
-              for (int k = 0; k < 8; ++k) as[k] = k == g.index ? 0 : (int)kStampEmpty;   // own AcceptOk (:781-789)
-              ep_store8(l + L_ASTAMP, as);
-              l[L_KIND] = LK_ACCEPTING;
+              ep_slow_path(g, l, c, h0, ans, in, o);
             }
           }
         }
@@ -600,6 +679,238 @@ __global__ void __launch_bounds__(kEpTile) ep_response_decide_kernel(EpParams P,
   __syncthreads();
   int32_t* dst = P.out + tile0 * WO;
   for (int e = tid; e < rows * WO; e += kEpTile) __stcs(dst + e, s_out[e]);
+}
+
+// =========================================================================== recovery and the control path
+// Reply rows staged in shared memory with an odd row stride WOp (conflict-free when thread t writes row t) leave
+// as one coalesced span of rows * WO words.
+__device__ __forceinline__ void ep_store_rows(int32_t* dst, const int32_t* s_out, int rows, int WO, int WOp) {
+  for (int e = threadIdx.x; e < rows * WO; e += kEpTile) {
+    const int row = e / WO;
+    __stcs(dst + e, s_out[row * WOp + (e - row * WO)]);
+  }
+}
+// one atomicMax per CTA of a per-thread ballot key
+__device__ __forceinline__ void ep_cta_max(unsigned long long m, unsigned long long* dst) {
+  __shared__ unsigned long long s_big[kEpTile / 32];
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, d));
+  if ((threadIdx.x & 31) == 0) s_big[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int w = 1; w < kEpTile / 32; ++w) m = max(m, s_big[w]);
+    if (m) atomicMax(dst, m);
+  }
+}
+
+// ---- handleCommit (:1567-1575) -> commit (:815-831).  in row: {rep, num, value, seq, deps[n]}; no reply.
+// CommittedEntry(triple) whatever the entry held (:826-827) and no leader state of any kind (:831).
+__global__ void __launch_bounds__(kEpTile) ep_commit_kernel(EpParams P) {
+  const EpGeometry& g = P.g;
+  extern __shared__ int32_t s_ep[];
+  const int W = 4 + g.n, Wp = W | 1;
+  const int tid = threadIdx.x;
+  const long long tile0 = (long long)blockIdx.x * kEpTile;
+  const int rows = (int)min((long long)kEpTile, P.n_rec - tile0);
+  ep_stage_rows(P.in, tile0, rows, W, Wp, s_ep);
+  __syncthreads();
+  if (tid >= rows) return;
+  const int i = (int)tile0 + tid;
+  const int32_t* r = s_ep + tid * Wp;
+  const long long inst = ep_instance(g, r[0], r[1]);
+  if (inst < 0) {
+    report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
+  } else if (!ep_claim(P.s, inst, P.tag, i)) {
+    int dd[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) dd[k] = k < g.n ? r[4 + k] : 0;
+    int4* c4 = (int4*)(P.s.cmd + inst * kEpCmdWords);
+    __stcg(c4, make_int4(EK_COMMITTED, r[2], -1, -1));
+    __stcg(c4 + 1, make_int4(-1, -1, r[3], 0));
+    __stcg(c4 + 2, make_int4(dd[0], dd[1], dd[2], dd[3]));
+    __stcg(c4 + 3, make_int4(dd[4], dd[5], dd[6], dd[7]));
+    P.s.lead[inst * kEpLeadWords + L_KIND] = LK_NONE;
+  }
+}
+
+// ---- handleNack (:1577-1630).  in row: {rep, num, lb_ord, lb_rep}; out row: {kind}.  Every Nack raises
+// largestBallot (:1578; a max, so the batch order does not matter); RECOVER_TIMER when a leader state of any kind
+// has a ballot below the Nack's (:1580-1618), i.e. the caller (re)arms the recoverInstance timer (:1623-1629).
+__global__ void __launch_bounds__(kEpTile) ep_nack_kernel(EpParams P) {
+  const EpGeometry& g = P.g;
+  extern __shared__ int32_t s_ep[];
+  const int W = 4, Wp = W | 1;
+  const int tid = threadIdx.x;
+  const long long tile0 = (long long)blockIdx.x * kEpTile;
+  const int rows = (int)min((long long)kEpTile, P.n_rec - tile0);
+  ep_stage_rows(P.in, tile0, rows, W, Wp, s_ep);
+  __syncthreads();
+  unsigned long long seen = 0;
+  if (tid < rows) {
+    const int i = (int)tile0 + tid;
+    const int32_t* r = s_ep + tid * Wp;
+    int kind = EV_NONE;
+    const long long inst = ep_instance(g, r[0], r[1]);
+    if (inst < 0) {
+      report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
+    } else {
+      seen = ballot_key(r[2], r[3]);
+      const int4 lh = __ldcg((const int4*)(P.s.lead + inst * kEpLeadWords));   // {kind, value, bord, brep}
+      if (lh.x != LK_NONE && ballot_key(lh.z, lh.w) < seen) kind = EV_RECOVER_TIMER;
+    }
+    __stcs(P.out + i, kind);
+  }
+  ep_cta_max(seen, P.s.largest);
+}
+
+// ---- transitionToPreparePhase (:969-996).  in row: {rep, num}; out row: {b_ord, b_rep}, the ballot of the
+// Prepare to send.  largestBallot is read floored at (0, index) (its initial value in the reference, :458): row i
+// gets (L + 1 + i, index), L the floored ordering at call start, and each transition raises largestBallot in
+// turn (:976).  The row's leader state becomes Preparing in that ballot with no responses (the replica's own
+// PrepareOk arrives as a message, :985); cmdLog is not touched.
+__global__ void __launch_bounds__(kEpTile) ep_prepare_phase_kernel(EpParams P) {
+  const EpGeometry& g = P.g;
+  const int i = blockIdx.x * kEpTile + threadIdx.x;
+  int L, rep;
+  key_ballot(max(__ldcg(P.s.largest), ballot_key(0, g.index)), L, rep);
+  unsigned long long seen = 0;
+  if (i < P.n_rec) {
+    const int2 r = __ldcs((const int2*)P.in + i);
+    const long long ord = (long long)L + 1 + i;
+    int2 out = make_int2(-1, -1);
+    const long long inst = ep_instance(g, r.x, r.y);
+    if (inst < 0) {
+      report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
+    } else if (ord > FPX_MAX_ROUND) {
+      report_error(P.s.st, FPX_ERR_ROUND_RANGE, i);
+    } else if (!ep_claim(P.s, inst, P.tag, i)) {
+      int4* l4 = (int4*)(P.s.lead + inst * kEpLeadWords);
+      const int4 empty = make_int4((int)kStampEmpty, (int)kStampEmpty, (int)kStampEmpty, (int)kStampEmpty);
+      __stcg(l4, make_int4(LK_PREPARING, 0, (int)ord, g.index));
+      __stcg(l4 + 1, make_int4(0, 0, 0, 0));
+      __stcg(l4 + L_ASTAMP / 4, empty); __stcg(l4 + L_ASTAMP / 4 + 1, empty);
+      __stcg(l4 + L_RSTAMP / 4, empty); __stcg(l4 + L_RSTAMP / 4 + 1, empty);
+      out = make_int2((int)ord, g.index);
+      seen = ballot_key((int)ord, g.index);
+    }
+    __stcs((int2*)P.out + i, out);
+  }
+  ep_cta_max(seen, P.s.largest + 1);
+}
+
+// ---- handlePrepare (:1632-1757).  in row: {rep, num, b_ord, b_rep}
+// out row: {kind, yielded, b_ord, b_rep, vb_ord, vb_rep, status, value, seq, deps[n]} -- PrepareOk (kind OK,
+// b = the Prepare's ballot), Nack (kind NACK, b = largestBallot, filled by the fix-up pass), Commit (kind COMMIT,
+// the triple).  Fields a reply does not carry are (-1, -1) ballots and zeros.
+__global__ void __launch_bounds__(kEpTile) ep_prepare_kernel(EpParams P) {
+  const EpGeometry& g = P.g;
+  extern __shared__ int32_t s_ep[];
+  const int W = 4, Wp = W | 1, WO = 9 + g.n, WOp = WO | 1;
+  int32_t* s_out = s_ep + kEpTile * Wp;
+  const int tid = threadIdx.x;
+  const long long tile0 = (long long)blockIdx.x * kEpTile;
+  const int rows = (int)min((long long)kEpTile, P.n_rec - tile0);
+  ep_stage_rows(P.in, tile0, rows, W, Wp, s_ep);
+  __syncthreads();
+  unsigned long long seen = 0;
+  if (tid < rows) {
+    const int i = (int)tile0 + tid;
+    const int32_t* r = s_ep + tid * Wp;
+    int32_t* o = s_out + tid * WOp;
+    o[0] = REPLY_NONE; o[1] = 0; o[2] = -1; o[3] = -1; o[4] = -1; o[5] = -1; o[6] = ST_NOT_SEEN; o[7] = 0; o[8] = 0;
+    for (int k = 0; k < g.n; ++k) o[9 + k] = 0;
+    const long long inst = ep_instance(g, r[0], r[1]);
+    if (inst < 0) {
+      report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
+    } else if (!ep_claim(P.s, inst, P.tag, i)) {
+      const unsigned long long b = ballot_key(r[2], r[3]);
+      seen = b;                                                 // largestBallot = max(.., prepare.ballot) (:1637)
+      int32_t* l = P.s.lead + inst * kEpLeadWords;
+      const int4 lh = __ldcg((const int4*)l);                   // {kind, value, bord, brep}
+      if (lh.x != LK_NONE && b > ballot_key(lh.z, lh.w)) {      // yield, before the stale check (:1645-1649)
+        l[L_KIND] = LK_NONE;
+        o[1] = 1;
+      }
+      int4* c4 = (int4*)(P.s.cmd + inst * kEpCmdWords);
+      const int4 h0 = __ldcg(c4), h1 = __ldcg(c4 + 1);          // {kind, value, bord, brep} {vbord, vbrep, seq, pad}
+      const int kind = h0.x;
+      if (kind == EK_COMMITTED || kind == EK_PREACCEPTED || kind == EK_ACCEPTED) {
+        const int4 d0 = __ldcg(c4 + 2), d1 = __ldcg(c4 + 3);
+        const int dd[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
+        for (int k = 0; k < g.n; ++k) o[9 + k] = dd[k];
+        o[7] = h0.y; o[8] = h1.z;
+      }
+      if (kind == EK_COMMITTED) {                               // :1746-1755 reply Commit(triple)
+        o[0] = REPLY_COMMIT;
+      } else if (kind != EK_NONE && b < ballot_key(h0.z, h0.w)) {   // :1676-1679 / :1700-1703 / :1724-1727
+        o[0] = REPLY_NACK;
+        o[7] = 0; o[8] = 0;
+        for (int k = 0; k < g.n; ++k) o[9 + k] = 0;
+        atomicOr(&P.s.st->ts_flags, 1u);                        // this batch needs the fix-up
+      } else {
+        o[0] = REPLY_OK; o[2] = r[2]; o[3] = r[3];
+        if (kind == EK_PREACCEPTED || kind == EK_ACCEPTED) {    // :1705-1720 / :1729-1744
+          o[4] = h1.x; o[5] = h1.y; o[6] = kind == EK_PREACCEPTED ? ST_PRE_ACCEPTED : ST_ACCEPTED;
+          __stcg(c4, make_int4(kind, h0.y, r[2], r[3]));        // entry.copy(ballot = prepare.ballot)
+        } else {                                                // NoCommandEntry(prepare.ballot) (:1669 / :1696)
+          __stcg(c4, make_int4(EK_NOCOMMAND, 0, r[2], r[3]));
+          __stcg(c4 + 1, make_int4(-1, -1, 0, 0));
+          __stcg(c4 + 2, make_int4(0, 0, 0, 0));
+          __stcg(c4 + 3, make_int4(0, 0, 0, 0));
+        }
+      }
+    }
+    P.s.proc_ballot[i] = seen;
+  }
+  ep_cta_max(seen, P.s.largest + 1);
+  __syncthreads();
+  ep_store_rows(P.out + tile0 * WO, s_out, rows, WO, WOp);
+}
+
+// ---- the defaultToSlowPath timer (:1015-1036) -> preAcceptingSlowPath (:796-813).  in row: {rep, num, b_ord,
+// b_rep}; out row as PreAcceptOk events {kind, seq, deps[n]}.  Only a row still PreAccepting in that ballot with
+// the timer armed (LF_TIMER, set where EV_TIMER was emitted) takes the slow path, over every answer it holds; in
+// any other state the reference's stopTimers (:618-630) has cancelled the timer and the event is NONE.
+__global__ void __launch_bounds__(kEpTile) ep_slow_path_timer_kernel(EpParams P) {
+  const EpGeometry& g = P.g;
+  extern __shared__ int32_t s_ep[];
+  const int W = 4, Wp = W | 1, WO = 2 + g.n;                    // odd: conflict-free as it is
+  int32_t* s_out = s_ep + kEpTile * Wp;
+  const int tid = threadIdx.x;
+  const long long tile0 = (long long)blockIdx.x * kEpTile;
+  const int rows = (int)min((long long)kEpTile, P.n_rec - tile0);
+  ep_stage_rows(P.in, tile0, rows, W, Wp, s_ep);
+  __syncthreads();
+  if (tid < rows) {
+    const int i = (int)tile0 + tid;
+    const int32_t* r = s_ep + tid * Wp;
+    int32_t* o = s_out + tid * WO;
+    for (int k = 0; k < WO; ++k) o[k] = 0;                      // o[0] = EV_NONE
+    const long long inst = ep_instance(g, r[0], r[1]);
+    if (inst < 0) {
+      report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
+    } else if (!ep_claim(P.s, inst, P.tag, i)) {
+      int32_t* l = P.s.lead + inst * kEpLeadWords;
+      int32_t* c = P.s.cmd + inst * kEpCmdWords;
+      const int4 h0 = __ldcg((const int4*)l);                   // {kind, value, bord, brep}
+      if (h0.x == LK_PREACCEPTING && ballot_key(r[2], r[3]) == ballot_key(h0.z, h0.w) &&
+          (__ldcg(&l[L_FLAGS]) & LF_TIMER)) {
+        int st[8];
+        ep_load8(l + L_RSTAMP, st);
+        int ans[kEpMaxN - 1][8];
+        bool in[kEpMaxN - 1];
+#pragma unroll
+        for (int a = 0; a < kEpMaxN - 1; ++a) {
+          in[a] = a < g.n && (uint32_t)st[a] != kStampEmpty;
+          if (in[a]) ep_load8(l + L_RESP + a * kEpRespWords, ans[a]);
+        }
+        ep_slow_path(g, l, c, h0, ans, in, o);
+      }
+    }
+  }
+  __syncthreads();
+  ep_store_rows(P.out + tile0 * WO, s_out, rows, WO, WO);
 }
 
 // ---- dense dep-set union (all `values` empty): elementwise max over the R sets of a group.

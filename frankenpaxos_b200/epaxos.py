@@ -10,6 +10,11 @@ from .engine import FpxError
 
 REPLY_NONE, REPLY_OK, REPLY_NACK, REPLY_COMMIT = 0, 1, 2, 3
 EV_NONE, EV_FAST_COMMIT, EV_SLOW_ACCEPT, EV_TIMER, EV_COMMIT = 0, 1, 2, 3, 4
+EV_RECOVER_TIMER = 1    # nack(): (re)arm the instance's recoverInstance timer
+EV_RESTART = 1          # prepareok(): run lead(avoid_fast_path = 1) in the returned ballot with the returned value
+LEADER_NONE, LEADER_PREACCEPTING, LEADER_ACCEPTING, LEADER_PREPARING = 0, 1, 2, 3
+STATUS_NOT_SEEN, STATUS_PRE_ACCEPTED, STATUS_ACCEPTED = 0, 1, 2
+VALUE_NOOP = -(1 << 31)
 
 
 class EpaxosConfig(C.Structure):
@@ -38,6 +43,16 @@ def _bind(L):
         f = getattr(L, nm)
         f.argtypes = [vp, vp, i32, vp]; f.restype = i32
     L.fpx_epaxos_preaccept_sets.argtypes = [vp, vp, i32, vp, vp, p(C.c_int64)]; L.fpx_epaxos_preaccept_sets.restype = i32
+    L.fpx_epaxos_commit.argtypes = [vp, vp, i32, p(C.c_int64)]; L.fpx_epaxos_commit.restype = i32
+    for nm in ("fpx_epaxos_nack", "fpx_epaxos_prepare_phase", "fpx_epaxos_prepare", "fpx_epaxos_prepareok",
+               "fpx_epaxos_slow_path_timer"):
+        f = getattr(L, nm)
+        f.argtypes = [vp, vp, i32, vp, p(C.c_int64)]; f.restype = i32
+    L.fpx_epaxos_commit_dev.argtypes = [vp, vp, i32]; L.fpx_epaxos_commit_dev.restype = i32
+    for nm in ("fpx_epaxos_nack_dev", "fpx_epaxos_prepare_phase_dev", "fpx_epaxos_prepare_dev",
+               "fpx_epaxos_prepareok_dev", "fpx_epaxos_slow_path_timer_dev"):
+        f = getattr(L, nm)
+        f.argtypes = [vp, vp, i32, vp]; f.restype = i32
     L._ep_bound = True
 
 
@@ -95,6 +110,33 @@ class EpaxosReplica:
     def acceptok(self, rows):
         return self._call(self._L.fpx_epaxos_acceptok, rows, 6, 2 + self.n)
 
+    # -- recovery and the timer-driven transitions (include/fpx.h)
+    def commit(self, rows):
+        """rows: {inst_replica, inst_number, value_id, seq, deps[n]} (handleCommit); no reply"""
+        self._call(self._L.fpx_epaxos_commit, rows, 4 + self.n, 0)
+
+    def nack(self, rows):
+        """rows: {inst_replica, inst_number, lb_ord, lb_rep} -> events {kind} (EV_RECOVER_TIMER)"""
+        return self._call(self._L.fpx_epaxos_nack, rows, 4, 1)
+
+    def prepare_phase(self, rows):
+        """rows: {inst_replica, inst_number} -> {b_ord, b_rep}, the ballot of the Prepare to send"""
+        return self._call(self._L.fpx_epaxos_prepare_phase, rows, 2, 2)
+
+    def prepare(self, rows):
+        """rows: {inst_replica, inst_number, b_ord, b_rep}
+        -> replies {kind, yielded, b_ord, b_rep, vb_ord, vb_rep, status, value_id, seq, deps[n]}"""
+        return self._call(self._L.fpx_epaxos_prepare, rows, 4, 9 + self.n)
+
+    def prepareok(self, rows):
+        """rows: {inst_replica, inst_number, b_ord, b_rep, from, vb_ord, vb_rep, status, value_id}
+        -> events {kind, b_ord, b_rep, value_id} (EV_RESTART)"""
+        return self._call(self._L.fpx_epaxos_prepareok, rows, 9, 4)
+
+    def slow_path_timer(self, rows):
+        """rows: {inst_replica, inst_number, b_ord, b_rep} -> events {kind, seq, deps[n]} (EV_SLOW_ACCEPT)"""
+        return self._call(self._L.fpx_epaxos_slow_path_timer, rows, 4, 2 + self.n)
+
     def last_kernel_ms(self):
         return float(self._L.fpx_epaxos_last_kernel_ms(self.h))
 
@@ -130,6 +172,26 @@ class EpaxosReplica:
 
     def acceptok_dev(self, d_in, n, d_event):
         self._dev(self._L.fpx_epaxos_acceptok_dev, d_in, n, d_event)
+
+    def commit_dev(self, d_in, n):
+        st = self._L.fpx_epaxos_commit_dev(self.h, d_in, n)
+        if st != 0:
+            raise FpxError(st)
+
+    def nack_dev(self, d_in, n, d_event):
+        self._dev(self._L.fpx_epaxos_nack_dev, d_in, n, d_event)
+
+    def prepare_phase_dev(self, d_in, n, d_ballot):
+        self._dev(self._L.fpx_epaxos_prepare_phase_dev, d_in, n, d_ballot)
+
+    def prepare_dev(self, d_in, n, d_reply):
+        self._dev(self._L.fpx_epaxos_prepare_dev, d_in, n, d_reply)
+
+    def prepareok_dev(self, d_in, n, d_event):
+        self._dev(self._L.fpx_epaxos_prepareok_dev, d_in, n, d_event)
+
+    def slow_path_timer_dev(self, d_in, n, d_event):
+        self._dev(self._L.fpx_epaxos_slow_path_timer_dev, d_in, n, d_event)
 
     def preaccept_sets(self, rows, overflow_count):
         """handlePreAccept for possibly sparse sets: FPX_ERR_UNSUPPORTED at the first message that carries

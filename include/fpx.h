@@ -449,6 +449,10 @@ typedef struct {
 enum { FPX_EP_REPLY_NONE = 0, FPX_EP_REPLY_OK = 1, FPX_EP_REPLY_NACK = 2, FPX_EP_REPLY_COMMIT = 3 };
 enum { FPX_EP_EV_NONE = 0, FPX_EP_EV_FAST_COMMIT = 1, FPX_EP_EV_SLOW_ACCEPT = 2, FPX_EP_EV_TIMER = 3,
        FPX_EP_EV_COMMIT = 4 };
+enum { FPX_EP_EV_RECOVER_TIMER = 1 };   /* fpx_epaxos_nack */
+enum { FPX_EP_EV_RESTART = 1 };         /* fpx_epaxos_prepareok */
+enum { FPX_EP_LEADER_NONE = 0, FPX_EP_LEADER_PREACCEPTING = 1, FPX_EP_LEADER_ACCEPTING = 2, FPX_EP_LEADER_PREPARING = 3 };
+enum { FPX_EP_STATUS_NOT_SEEN = 0, FPX_EP_STATUS_PRE_ACCEPTED = 1, FPX_EP_STATUS_ACCEPTED = 2 };
 
 int fpx_epaxos_create(fpx_epaxos** out, const fpx_epaxos_config* cfg);
 void fpx_epaxos_destroy(fpx_epaxos* e);
@@ -490,9 +494,63 @@ int fpx_epaxos_acceptok_dev(fpx_epaxos* e, const int32_t* d_in, int32_t n_rec, i
  * nothing of the batch is applied); union such sets with fpx_depset_union on the side. */
 int fpx_epaxos_preaccept_sets(fpx_epaxos* e, const int32_t* in, int32_t n_rec, const int32_t* overflow_count,
                               int32_t* reply, int64_t* err_index);
+
+/* Recovery and the timer-driven transitions (Replica.scala:969-1078, 1567-1869).  Same conventions as above:
+ * dense replies / events, first offending index, a _dev form asynchronous on fpx_epaxos_stream.  The caller keeps
+ * the timers, thrifty recipient choice, the conflict index and execution.  Wherever these calls read
+ * largestBallot they read max(largestBallot, (0, replica_index)), the reference's initial value (:458); the
+ * stored value starts at (-1, -1), as the existing handlers expect.
+ *
+ * handleCommit -> commit, :1567-1575, :815-831.  in rows of 4+n ints: {inst_replica, inst_number, value_id, seq,
+ * deps[n]}.  Writes CommittedEntry whatever the entry held, even an earlier Committed one, and drops the
+ * instance's leader state of any kind.  No reply.  Batch contract E1.  The caller still updates the conflict
+ * index (fpx_conflict_index_batch mode PUT) and commits to the dependency graph. */
+int fpx_epaxos_commit(fpx_epaxos* e, const int32_t* in, int32_t n_rec, int64_t* err_index);
+/* handleNack, :1577-1630.  in rows of 4 ints: {inst_replica, inst_number, lb_ord, lb_rep}; event rows of 1 int:
+ * RECOVER_TIMER when this replica leads the instance (any leader kind, Preparing included) in a ballot below the
+ * Nack's: (re)arm the recoverInstance timer.  Every Nack raises largestBallot.  No batch contract. */
+int fpx_epaxos_nack(fpx_epaxos* e, const int32_t* in, int32_t n_rec, int32_t* event, int64_t* err_index);
+/* transitionToPreparePhase, :969-996 (the recoverInstance timer fired).  in rows of 2 ints: {inst_replica,
+ * inst_number}; out rows of 2 ints: {b_ord, b_rep}, the ballot of the Prepare to send, to f other replicas and
+ * to this one.  Row i gets (L + 1 + i, replica_index), L = the floored largestBallot's ordering at call start;
+ * each row raises largestBallot.  The leader state becomes Preparing with no responses; cmdLog is untouched.
+ * An ordering past FPX_MAX_ROUND is FPX_ERR_ROUND_RANGE.  Batch contract E1. */
+int fpx_epaxos_prepare_phase(fpx_epaxos* e, const int32_t* in, int32_t n_rec, int32_t* ballot, int64_t* err_index);
+/* handlePrepare, :1632-1757.  in rows of 4 ints: {inst_replica, inst_number, b_ord, b_rep}; reply rows of 9+n
+ * ints: {kind, yielded, b_ord, b_rep, vb_ord, vb_rep, status, value_id, seq, deps[n]}, status 0 NotSeen 1
+ * PreAccepted 2 Accepted.  kind OK = PrepareOk in the Prepare's ballot (NotSeen with a (-1, -1) vote ballot and
+ * no triple for an absent or NoCommand entry), NACK = Nack(largestBallot) in b, COMMIT = Commit(triple); fields a
+ * reply does not carry are (-1, -1) and 0.  Every Prepare raises largestBallot BEFORE the Nack is built (:1637,
+ * :1652): the Nack of message i carries the max over the handle's value before the call and messages 0..i.
+ * yielded = 1 when the Prepare's ballot exceeded this replica's leader ballot (any kind) and the leader state was
+ * dropped -- also for a Nacked Prepare; stop that instance's timers.  Batch contract E1. */
+int fpx_epaxos_prepare(fpx_epaxos* e, const int32_t* in, int32_t n_rec, int32_t* reply, int64_t* err_index);
+/* handlePrepareOk, :1759-1869.  in rows of 9 ints: {inst_replica, inst_number, b_ord, b_rep, from_replica,
+ * vb_ord, vb_rep, status, value_id} (a PrepareOk's seq and deps are not inputs: no reachable branch reads them);
+ * event rows of 4 ints: {kind, b_ord, b_rep, value_id}.  Counted only while the leader state is Preparing in
+ * that ballot; a larger ballot is FPX_ERR_CHECK_FAILED (logger.checkLt, :1792).  At the delivery that completes
+ * f+1 responses: among those with the maximum vote ballot, the PreAccepted one of the lowest replica index gives
+ * value_id, else FPX_VALUE_NOOP; kind RESTART, and the instance is led by nobody until the caller runs the
+ * conflict index (mode 0) and fpx_epaxos_lead with avoid_fast_path = 1 in {b_ord, b_rep} -- which it must do
+ * before its next call that touches these instances (transitionToPreAcceptPhase, :1856-1867).  An Accepted
+ * response is never re-accepted and the fast-path candidates are never taken: both branches are unreachable in
+ * the reference (:1813, :1836) and stay so.  Batch contract E2. */
+int fpx_epaxos_prepareok(fpx_epaxos* e, const int32_t* in, int32_t n_rec, int32_t* event, int64_t* err_index);
+/* The defaultToSlowPath timer fired (:1015-1036) -> preAcceptingSlowPath (:796-813).  in rows of 4 ints:
+ * {inst_replica, inst_number, b_ord, b_rep} (the ballot the timer was armed in); event rows as PreAcceptOk's:
+ * SLOW_ACCEPT {seq, deps} over every answer the leader holds, when it is still PreAccepting in that ballot with the
+ * timer armed by an earlier TIMER event; NONE otherwise (the reference would have stopped the timer).  E1. */
+int fpx_epaxos_slow_path_timer(fpx_epaxos* e, const int32_t* in, int32_t n_rec, int32_t* event, int64_t* err_index);
+int fpx_epaxos_commit_dev(fpx_epaxos* e, const int32_t* d_in, int32_t n_rec);
+int fpx_epaxos_nack_dev(fpx_epaxos* e, const int32_t* d_in, int32_t n_rec, int32_t* d_event);
+int fpx_epaxos_prepare_phase_dev(fpx_epaxos* e, const int32_t* d_in, int32_t n_rec, int32_t* d_ballot);
+int fpx_epaxos_prepare_dev(fpx_epaxos* e, const int32_t* d_in, int32_t n_rec, int32_t* d_reply);
+int fpx_epaxos_prepareok_dev(fpx_epaxos* e, const int32_t* d_in, int32_t n_rec, int32_t* d_event);
+int fpx_epaxos_slow_path_timer_dev(fpx_epaxos* e, const int32_t* d_in, int32_t n_rec, int32_t* d_event);
+
 /* read-back: out[7+n] = {kind, b_ord, b_rep, vb_ord, vb_rep, value_id, seq, deps[n]},
  * kind 0 none 1 NoCommand 2 PreAccepted 3 Accepted 4 Committed; *leader_kind 0 none 1
- * PreAccepting 2 Accepting; largest_ballot[2] */
+ * PreAccepting 2 Accepting 3 Preparing; largest_ballot[2] (as stored: (-1, -1) before any ballot) */
 /* device time (ms, CUDA events on the handle's stream) of the kernels of the last
  * fpx_epaxos_* call, without its host<->device copies */
 float fpx_epaxos_last_kernel_ms(fpx_epaxos* e);
