@@ -12,6 +12,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
 #include <new>
 #include <string>
 #include <vector>
@@ -22,6 +23,7 @@
 #include "fpx_conflict.cuh"
 #include "fpx_depgraph.cuh"
 #include "fpx_epaxos.cuh"
+#include "fpx_host.h"
 #include "fpx_ranges.cuh"
 #include "fpx_reads.cuh"
 #include "fpx_replica_misc.cuh"
@@ -39,6 +41,7 @@ constexpr int kStepRing = 1024;
 constexpr int32_t kTallyMaxSub = (40 * 1024 / 4) * kChunkVotes;
 
 struct fpx_engine {
+  CudaResources res;                   // every buffer, stream and event below
   fpx_config cfg;
   Geometry g;
   cudaStream_t stream = nullptr;
@@ -62,7 +65,7 @@ struct fpx_engine {
   uint32_t rng_seq_base = 1;               // Phase2bNoopRange delivery sequence numbers
   int unit_ranges = 0;                     // a one-slot range was ever armed: arms must look at the range keys
   // fpx_step_dev: CUDA events around the acceptor and tally kernels of the last kStepRing steps
-  cudaEvent_t* step_ev = nullptr;          // [kStepRing][3], created on first use
+  std::vector<cudaEvent_t> step_ev;        // [kStepRing][4], created on first use
   // wire codec staging (grown on demand)
   struct WireBuf { void* p = nullptr; size_t cap = 0; };
   WireBuf w_bytes, w_offs, w_kind, w_rec, w_out, w_tiles, w_arena, w_voffs;
@@ -99,6 +102,7 @@ struct fpx_engine {
     DevStatus* h_st = nullptr;
     fpx_p2b* out_p2b = nullptr; fpx_nack* out_nack = nullptr; fpx_chosen* out_chosen = nullptr;
     int32_t n_p2a = 0;
+    bool ready = false;                // every resource above exists
     bool busy = false;
   } lane[2];
   int lane_head = 0, lane_tail = 0, lanes_in_flight = 0;
@@ -116,14 +120,61 @@ struct fpx_engine {
   std::string last_error;
 };
 
-#define CK(e, call)                                                              \
-  do {                                                                           \
-    cudaError_t _err = (call);                                                   \
-    if (_err != cudaSuccess) {                                                   \
-      (e)->last_error = std::string(#call) + ": " + cudaGetErrorString(_err);   \
-      return FPX_ERR_CUDA;                                                       \
-    }                                                                            \
-  } while (0)
+// --------------------------------------------------------------------------- status blocks (DevStatus, ReadsDev)
+
+// a fresh status block: no error, every other field 0
+template <class S>
+static S fresh_status() {
+  S st;
+  memset(&st, 0, sizeof(S));
+  st.err_word = ~0ull;
+  return st;
+}
+
+// writes `init` to the device's status block through the pinned mirror
+template <class H, class S>
+static int status_init(H* h, S* hs, S* ds, cudaStream_t s, const S& init = fresh_status<S>()) {
+  *hs = init;
+  CK(h, cudaMemcpyAsync(ds, hs, sizeof(S), cudaMemcpyHostToDevice, s));
+  CK(h, cudaStreamSynchronize(s));
+  return FPX_OK;
+}
+
+// The error word of a status block already copied to the host: *status is the first error's status (FPX_OK:
+// none) and *err_index its record (-1: none, or an error of the reads handle that belongs to no record).  The
+// word is cleared on the device (the reference process would be dead: cleared for the caller's reset), and the
+// clear waited for if `sync`.  Returns FPX_ERR_CUDA if the clear failed, else FPX_OK.
+template <class H, class S>
+static int take_error(H* h, const S& hs, S* ds, cudaStream_t s, bool sync, int* status, int64_t* err_index) {
+  const unsigned long long w = hs.err_word;
+  *status = FPX_OK;
+  if (err_index) *err_index = -1;
+  if (w == ~0ull) return FPX_OK;
+  long long idx = (long long)(w >> 8);
+  if constexpr (std::is_same<S, ReadsDev>::value) idx = idx == kRdNoIndex ? -1 : idx;
+  if (err_index) *err_index = idx;
+  *status = -(int)(w & 0xff);
+  const unsigned long long none = ~0ull;
+  CK(h, cudaMemcpyAsync(&ds->err_word, &none, 8, cudaMemcpyHostToDevice, s));
+  if (sync) CK(h, cudaStreamSynchronize(s));
+  return FPX_OK;
+}
+
+// copies the status block to its pinned mirror once the stream's work is done, and takes its error (take_error)
+template <class H, class S>
+static int read_status(H* h, S* hs, S* ds, cudaStream_t s, int* status, int64_t* err_index) {
+  CK(h, cudaMemcpyAsync(hs, ds, sizeof(S), cudaMemcpyDeviceToHost, s));
+  CK(h, cudaStreamSynchronize(s));
+  return take_error(h, *hs, ds, s, true, status, err_index);
+}
+
+// read_status for callers that return either: FPX_ERR_CUDA if a CUDA call failed, else the block's status
+template <class H, class S>
+static int collect_status(H* h, S* hs, S* ds, cudaStream_t s, int64_t* err_index) {
+  int status = FPX_OK;
+  const int c = read_status(h, hs, ds, s, &status, err_index);
+  return c != FPX_OK ? c : status;
+}
 
 static int validate(const fpx_config* c) {
   // Config.checkValid, S/multipaxos/Config.scala:32-147 (clauses the path reads)
@@ -187,18 +238,15 @@ static int reset_state(fpx_engine* e) {
   if (e->rng_tab) CK(e, cudaMemsetAsync(e->rng_tab, 0xff, (size_t)e->rng_cap * kRangeWords * 4, e->stream));
   e->rng_seq_base = 1;
   e->unit_ranges = 0;
-  DevStatus init;
-  memset(&init, 0, sizeof(init));
-  init.err_word = ~0ull;
+  DevStatus init = fresh_status<DevStatus>();
   init.max_chosen_local = -1;
   init.max_armed_local = -1;
   init.wm_found = INT_MAX;
   init.ts_min_local = INT_MAX; init.ts_max_local = -1;
   init.ts_min_round = INT_MAX; init.ts_max_round = INT_MIN;
   init.watermark = g.shard_index;
-  *e->h_st = init;
-  CK(e, cudaMemcpyAsync(e->st, e->h_st, sizeof(DevStatus), cudaMemcpyHostToDevice, e->stream));
-  CK(e, cudaStreamSynchronize(e->stream));
+  int c = status_init(e, e->h_st, e->st, e->stream, init);
+  if (c != FPX_OK) return c;
   CK(e, cudaMemsetAsync(e->xch_table, 0, kMaxShards * 8, e->stream));
   e->h_xch.epoch = 0;
   e->xch_epoch = 0;
@@ -212,6 +260,22 @@ static int reset_state(fpx_engine* e) {
   e->rseq_base = 1;
   e->last_p2b_n = 0;
   return FPX_OK;
+}
+
+// The host form of a call on the staging buffer: `bytes` of `in` to d_in, `launch(d_in)`, then fpx_sync into *r
+// (a local one if null) and *err_index.
+template <class F>
+static int staged_call(fpx_engine* e, const void* in, size_t bytes, int64_t* err_index, fpx_sync_result* r, F launch) {
+  CK(e, cudaSetDevice(e->cfg.device));
+  CK(e, cudaMemcpyAsync(e->d_in, in, bytes, cudaMemcpyHostToDevice, e->stream));
+  int c = launch(e->d_in);
+  if (c != FPX_OK) return c;
+  fpx_sync_result local;
+  if (!r) r = &local;
+  r->err_index = -1;   // fpx_sync leaves *r alone when a CUDA call fails
+  c = fpx_sync(e, r);
+  if (err_index) *err_index = r->err_index;
+  return c;
 }
 
 extern "C" {
@@ -248,12 +312,12 @@ int fpx_create(fpx_engine** out, const fpx_config* cfg) {
   *out = nullptr;
   int v = validate(cfg);
   if (v != FPX_OK) return v;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return FPX_ERR_NO_DEVICE;
-  if (cfg->device < 0 || cfg->device >= ndev) return FPX_ERR_NO_DEVICE;
-  fpx_engine* e = new (std::nothrow) fpx_engine();
+  if (!device_exists(cfg->device)) return FPX_ERR_NO_DEVICE;
+  std::unique_ptr<fpx_engine> e(new (std::nothrow) fpx_engine());   // freed with all it holds on a failed return
   if (!e) return FPX_ERR_INVALID_ARG;
   e->cfg = *cfg;
+  CudaResources& R = e->res;
+  R.device = cfg->device;
   Geometry& g = e->g;
   g.protocol = cfg->protocol;
   g.f = cfg->f;
@@ -282,60 +346,51 @@ int fpx_create(fpx_engine** out, const fpx_config* cfg) {
   g.m_lgroups = ~0ull / (unsigned long long)g.lgroups + 1ull;
   g.m_agroups = ~0ull / (unsigned long long)g.agroups + 1ull;
 
-  auto fail = [&](int code) { fpx_destroy(e); return code; };
-#define CKC(call)                                                                \
-  do {                                                                           \
-    cudaError_t _err = (call);                                                   \
-    if (_err != cudaSuccess) {                                                   \
-      fprintf(stderr, "fpx_create: %s: %s\n", #call, cudaGetErrorString(_err)); \
-      return fail(FPX_ERR_CUDA);                                                 \
-    }                                                                            \
-  } while (0)
-  CKC(cudaSetDevice(cfg->device));
-  CKC(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
-  CKC(cudaStreamCreateWithFlags(&e->h2d_stream, cudaStreamNonBlocking));
-  CKC(cudaStreamCreateWithFlags(&e->d2h_stream, cudaStreamNonBlocking));
-  for (int i = 0; i < kMaxEvents; ++i) CKC(cudaEventCreateWithFlags(&e->ev[i], cudaEventDisableTiming));
+  CK(e, cudaSetDevice(cfg->device));
+  CK(e, R.stream(&e->stream));
+  CK(e, R.stream(&e->h2d_stream));
+  CK(e, R.stream(&e->d2h_stream));
+  for (int i = 0; i < kMaxEvents; ++i) CK(e, R.event(&e->ev[i], cudaEventDisableTiming));
   size_t mb = (size_t)cfg->max_batch;
-  CKC(cudaMalloc(&e->rows, (size_t)g.local_slots * g.row_words * 4));
+  CK(e, R.alloc(&e->rows, (size_t)g.local_slots * g.row_words * 4));
   if (g.ovf_cap) {
-    CKC(cudaMalloc(&e->ovf_keys, (size_t)g.ovf_cap * 8));
-    CKC(cudaMalloc(&e->ovf_rows, (size_t)g.ovf_cap * g.row_words * 4));
-    CKC(cudaMalloc(&e->ovf_keys_spare, (size_t)g.ovf_cap * 8));
-    CKC(cudaMalloc(&e->ovf_rows_spare, (size_t)g.ovf_cap * g.row_words * 4));
+    CK(e, R.alloc(&e->ovf_keys, (size_t)g.ovf_cap * 8));
+    CK(e, R.alloc(&e->ovf_rows, (size_t)g.ovf_cap * g.row_words * 4));
+    CK(e, R.alloc(&e->ovf_keys_spare, (size_t)g.ovf_cap * 8));
+    CK(e, R.alloc(&e->ovf_rows_spare, (size_t)g.ovf_cap * g.row_words * 4));
   }
-  CKC(cudaMalloc(&e->votes, ((size_t)g.local_slots * g.voters * 8) << g.cell_shift));
-  CKC(cudaMalloc(&e->acc_round, kMaxKeys * 4));
-  CKC(cudaMalloc(&e->acc_max_voted, kMaxKeys * 4));
-  CKC(cudaMalloc(&e->rlog, (size_t)g.local_slots * 8));
+  CK(e, R.alloc(&e->votes, ((size_t)g.local_slots * g.voters * 8) << g.cell_shift));
+  CK(e, R.alloc(&e->acc_round, kMaxKeys * 4));
+  CK(e, R.alloc(&e->acc_max_voted, kMaxKeys * 4));
+  CK(e, R.alloc(&e->rlog, (size_t)g.local_slots * 8));
   if (cfg->protocol == FPX_MENCIUS) {
     e->rng_cap = std::max(1024, g.ovf_cap);
-    CKC(cudaMalloc(&e->rng_tab, (size_t)e->rng_cap * kRangeWords * 4));
-    CKC(cudaMalloc(&e->rng_tab_spare, (size_t)e->rng_cap * kRangeWords * 4));
+    CK(e, R.alloc(&e->rng_tab, (size_t)e->rng_cap * kRangeWords * 4));
+    CK(e, R.alloc(&e->rng_tab_spare, (size_t)e->rng_cap * kRangeWords * 4));
   }
-  if (cfg->protocol != FPX_MULTIPAXOS) CKC(cudaMalloc(&e->rng_dec, (size_t)(FPX_MAX_RANGE_BATCH + 1) * 4));
-  CKC(cudaMalloc(&e->st, sizeof(DevStatus)));
-  CKC(cudaMalloc(&e->xch, sizeof(DevExchange)));
-  CKC(cudaMalloc(&e->xch_table, kMaxShards * 8));
-  CKC(cudaMalloc(&e->xch_out, (1 + kMaxShards) * 4));
-  CKC(cudaMalloc(&e->bits, (mb / 32 + 2) * 4));
-  CKC(cudaMalloc(&e->g_agg, (size_t)2 * kMaxGrid * kMaxKeys * 4));
-  CKC(cudaMalloc(&e->g_wacc, (size_t)kAccMaxSegments * kMaxGrid * kAW * 4));
-  CKC(cudaMalloc(&e->t_bw, (mb / kChunkVotes + 2) * 32 * 8));
-  CKC(cudaMalloc(&e->t_cc, (mb / kChunkVotes + 2) * 4));
-  CKC(cudaMalloc(&e->t_tmp, (mb + kChunkVotes) * 8));   // padded to a whole chunk: phase D loads unconditionally
+  if (cfg->protocol != FPX_MULTIPAXOS) CK(e, R.alloc(&e->rng_dec, (size_t)(FPX_MAX_RANGE_BATCH + 1) * 4));
+  CK(e, R.alloc(&e->st, sizeof(DevStatus)));
+  CK(e, R.alloc(&e->xch, sizeof(DevExchange)));
+  CK(e, R.alloc(&e->xch_table, kMaxShards * 8));
+  CK(e, R.alloc(&e->xch_out, (1 + kMaxShards) * 4));
+  CK(e, R.alloc(&e->bits, (mb / 32 + 2) * 4));
+  CK(e, R.alloc(&e->g_agg, (size_t)2 * kMaxGrid * kMaxKeys * 4));
+  CK(e, R.alloc(&e->g_wacc, (size_t)kAccMaxSegments * kMaxGrid * kAW * 4));
+  CK(e, R.alloc(&e->t_bw, (mb / kChunkVotes + 2) * 32 * 8));
+  CK(e, R.alloc(&e->t_cc, (mb / kChunkVotes + 2) * 4));
+  CK(e, R.alloc(&e->t_tmp, (mb + kChunkVotes) * 8));   // padded to a whole chunk: phase D loads unconditionally
   {
     // cooperative (co-resident) grids: SMs x resident CTAs per SM
     cudaDeviceProp prop;
-    CKC(cudaGetDeviceProperties(&prop, cfg->device));
-    if (!prop.cooperativeLaunch) return fail(FPX_ERR_UNSUPPORTED);
+    CK(e, cudaGetDeviceProperties(&prop, cfg->device));
+    if (!prop.cooperativeLaunch) return FPX_ERR_UNSUPPORTED;
     e->num_sms = prop.multiProcessorCount;
     e->l2_bytes = prop.l2CacheSize;
     int occ = 0;
-    CKC(cudaFuncSetAttribute(acceptor_phase2a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (kMaxKeys + kAccMaxSegments) * kAT * 4));
-    CKC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, acceptor_phase2a_kernel, kAT,
-                                                      (size_t)(g.num_keys + kAccMaxSegments) * kAT * 4));
+    CK(e, cudaFuncSetAttribute(acceptor_phase2a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (kMaxKeys + kAccMaxSegments) * kAT * 4));
+    CK(e, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, acceptor_phase2a_kernel, kAT,
+                                                        (size_t)(g.num_keys + kAccMaxSegments) * kAT * 4));
     e->occ_acceptor = std::max(occ, 1);
     e->grid_acceptor = std::min(std::max(occ, 1) * e->num_sms, kMaxGrid);
     // the tally's dynamic shared memory: scan of the per-chunk counts (4 B per 1024 votes) + the CTA's kept
@@ -343,61 +398,35 @@ int fpx_create(fpx_engine** out, const fpx_config* cfg) {
     const int smem_cap = kTallySmem;
     e->tally_max_sub = kTallyMaxSub;
     const void* tk = tally_kernel_ptr(g.row_words);
-    CKC(cudaFuncSetAttribute(tk, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_cap));
-    CKC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, tk, kTT, smem_cap));
+    CK(e, cudaFuncSetAttribute(tk, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_cap));
+    CK(e, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, tk, kTT, smem_cap));
     e->occ_tally = std::max(occ, 1);
     e->grid_tally = std::min(std::max(occ, 1) * e->num_sms, kMaxGrid);
   }
-  CKC(cudaMalloc(&e->conflicts, kMaxConflicts * 8));
-  CKC(cudaMalloc(&e->arm_conflicts, kMaxConflicts * 8));
-  CKC(cudaMalloc(&e->arm_bits, (mb / 32 + 2) * 4));
-  CKC(cudaMalloc(&e->d_in, mb * 16));
-  CKC(cudaMalloc(&e->d_out_a, mb * 16));
-  CKC(cudaMalloc(&e->d_out_b, mb * 8));
-  CKC(cudaMallocHost(&e->h_st, sizeof(DevStatus)));
-#undef CKC
+  CK(e, R.alloc(&e->conflicts, kMaxConflicts * 8));
+  CK(e, R.alloc(&e->arm_conflicts, kMaxConflicts * 8));
+  CK(e, R.alloc(&e->arm_bits, (mb / 32 + 2) * 4));
+  CK(e, R.alloc(&e->d_in, mb * 16));
+  CK(e, R.alloc(&e->d_out_a, mb * 16));
+  CK(e, R.alloc(&e->d_out_b, mb * 8));
+  CK(e, R.alloc_pinned(&e->h_st, sizeof(DevStatus)));
   memset(&e->h_xch, 0, sizeof(e->h_xch));
   e->h_xch.n = g.shard_count <= kMaxShards ? g.shard_count : 0;
   e->h_xch.mine = g.shard_index;
   e->h_xch.tabs[g.shard_index < kMaxShards ? g.shard_index : 0] = g.shard_count <= kMaxShards ? e->xch_table : nullptr;
   e->h_xch.enabled = g.shard_count > 1 && g.shard_count <= kMaxShards;
-  int r = reset_state(e);
-  if (r != FPX_OK) { fprintf(stderr, "fpx_create: %s\n", e->last_error.c_str()); return fail(r); }
+  int r = reset_state(e.get());
+  if (r != FPX_OK) return r;
   // test / A-B knob: FPX_TALLY_PATH=exact makes every tally launch take the per-vote path
   if (const char* tp = getenv("FPX_TALLY_PATH")) e->tally_path = strcmp(tp, "exact") == 0 ? 2 : 0;
-  *out = e;
+  *out = e.release();
   return FPX_OK;
 }
 
 void fpx_destroy(fpx_engine* e) {
   if (!e) return;
-  cudaSetDevice(e->cfg.device);
-  if (e->stream) cudaStreamSynchronize(e->stream);
-  cudaFree(e->rows); cudaFree(e->ovf_keys); cudaFree(e->ovf_rows); cudaFree(e->votes);
-  cudaFree(e->ovf_keys_spare); cudaFree(e->ovf_rows_spare);
-  cudaFree(e->acc_round); cudaFree(e->acc_max_voted); cudaFree(e->rlog); cudaFree(e->st);
-  cudaFree(e->rng_tab); cudaFree(e->rng_tab_spare); cudaFree(e->rng_dec);
-  for (auto& ln : e->lane) {
-    cudaFree(ln.d_p2a); cudaFree(ln.d_p2b); cudaFree(ln.d_arm); cudaFree(ln.d_out_p2b); cudaFree(ln.d_out_nack); cudaFree(ln.d_out_chosen);
-    for (cudaEvent_t ev : {ln.ev_p2a, ln.ev_p2b, ln.ev_acc, ln.ev_done, ln.ev_d2h}) if (ev) cudaEventDestroy(ev);
-    if (ln.h_st) cudaFreeHost(ln.h_st);
-  }
-  for (int p = 0; p < kMaxShards; ++p) if (e->xch_opened[p]) cudaIpcCloseMemHandle(e->xch_opened[p]);
-  cudaFree(e->xch); cudaFree(e->xch_table); cudaFree(e->xch_out);
-  if (e->step_ev) {
-    for (int i = 0; i < kStepRing * 4; ++i) cudaEventDestroy(e->step_ev[i]);
-    delete[] e->step_ev;
-  }
-  for (fpx_engine::WireBuf* b : {&e->w_bytes, &e->w_offs, &e->w_kind, &e->w_rec, &e->w_out, &e->w_tiles, &e->w_arena,
-                                 &e->w_voffs})
-    cudaFree(b->p);
-  cudaFree(e->bits); cudaFree(e->g_agg); cudaFree(e->g_wacc); cudaFree(e->t_bw); cudaFree(e->t_cc); cudaFree(e->t_tmp); cudaFree(e->conflicts); cudaFree(e->arm_conflicts); cudaFree(e->arm_bits);
-  cudaFree(e->d_in); cudaFree(e->d_out_a); cudaFree(e->d_out_b);
-  if (e->h_st) cudaFreeHost(e->h_st);
-  for (int i = 0; i < kMaxEvents; ++i) if (e->ev[i]) cudaEventDestroy(e->ev[i]);
-  if (e->h2d_stream) cudaStreamDestroy(e->h2d_stream);
-  if (e->d2h_stream) cudaStreamDestroy(e->d2h_stream);
-  if (e->stream) cudaStreamDestroy(e->stream);
+  e->res.sync();   // no kernel reads a peer's table once its mapping is closed
+  for (void* p : e->xch_opened) if (p) cudaIpcCloseMemHandle(p);
   delete e;
 }
 
@@ -722,12 +751,12 @@ int fpx_step_dev(fpx_engine* e, const fpx_p2a* d_arm, int32_t n_arm, const fpx_p
   if (!e) return FPX_ERR_INVALID_ARG;
   cudaEvent_t* ev = nullptr;
   if (ring_slot >= 0) {
-    if (!e->step_ev) {
-      e->step_ev = new (std::nothrow) cudaEvent_t[kStepRing * 4];
-      if (!e->step_ev) return FPX_ERR_INVALID_ARG;
-      for (int i = 0; i < kStepRing * 4; ++i) CK(e, cudaEventCreate(&e->step_ev[i]));
+    if (e->step_ev.empty()) {   // all or nothing: a failed attempt's events stay with the owner until destroy
+      std::vector<cudaEvent_t> ring(kStepRing * 4);
+      for (cudaEvent_t& x : ring) CK(e, e->res.event(&x, cudaEventDefault));
+      e->step_ev.swap(ring);
     }
-    ev = e->step_ev + (size_t)(ring_slot % kStepRing) * 4;
+    ev = e->step_ev.data() + (size_t)(ring_slot % kStepRing) * 4;
   }
   // The arm batch and the acceptor batch touch disjoint state (proxy-leader rows / vote cells), so their
   // order is free; the acceptors go first so that the rows armed last are still L2-resident when the
@@ -748,8 +777,8 @@ int fpx_step_dev(fpx_engine* e, const fpx_p2a* d_arm, int32_t n_arm, const fpx_p
 }
 
 int fpx_step_kernel_ms(fpx_engine* e, int32_t ring_slot, float* acceptor_ms, float* tally_ms) {
-  if (!e || !e->step_ev || ring_slot < 0 || !acceptor_ms || !tally_ms) return FPX_ERR_INVALID_ARG;
-  cudaEvent_t* ev = e->step_ev + (size_t)(ring_slot % kStepRing) * 4;
+  if (!e || e->step_ev.empty() || ring_slot < 0 || !acceptor_ms || !tally_ms) return FPX_ERR_INVALID_ARG;
+  cudaEvent_t* ev = e->step_ev.data() + (size_t)(ring_slot % kStepRing) * 4;
   CK(e, cudaEventSynchronize(ev[3]));
   CK(e, cudaEventElapsedTime(acceptor_ms, ev[0], ev[1]));
   CK(e, cudaEventElapsedTime(tally_ms, ev[2], ev[3]));
@@ -758,14 +787,18 @@ int fpx_step_kernel_ms(fpx_engine* e, int32_t ring_slot, float* acceptor_ms, flo
 
 // --------------------------------------------------------------------------- asynchronous host step
 
+// A lane is ready once all of its resources exist; the pieces of a failed attempt stay with the owner until
+// destroy, and the next fpx_step_submit tries the whole set again.
 static int lane_init(fpx_engine* e, fpx_engine::Lane& ln) {
-  if (ln.d_p2a) return FPX_OK;
+  if (ln.ready) return FPX_OK;
   size_t mb = (size_t)e->cfg.max_batch;
-  CK(e, cudaMalloc(&ln.d_p2a, mb * 16)); CK(e, cudaMalloc(&ln.d_p2b, mb * 16)); CK(e, cudaMalloc(&ln.d_arm, mb * 16));
-  CK(e, cudaMalloc(&ln.d_out_p2b, mb * 16)); CK(e, cudaMalloc(&ln.d_out_nack, mb * 8)); CK(e, cudaMalloc(&ln.d_out_chosen, mb * 8));
+  CudaResources& R = e->res;
+  CK(e, R.alloc(&ln.d_p2a, mb * 16)); CK(e, R.alloc(&ln.d_p2b, mb * 16)); CK(e, R.alloc(&ln.d_arm, mb * 16));
+  CK(e, R.alloc(&ln.d_out_p2b, mb * 16)); CK(e, R.alloc(&ln.d_out_nack, mb * 8)); CK(e, R.alloc(&ln.d_out_chosen, mb * 8));
   for (cudaEvent_t* ev : {&ln.ev_p2a, &ln.ev_p2b, &ln.ev_acc, &ln.ev_done, &ln.ev_d2h})
-    CK(e, cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
-  CK(e, cudaMallocHost(&ln.h_st, sizeof(DevStatus)));
+    CK(e, R.event(ev, cudaEventDisableTiming));
+  CK(e, R.alloc_pinned(&ln.h_st, sizeof(DevStatus)));
+  ln.ready = true;
   return FPX_OK;
 }
 
@@ -819,14 +852,10 @@ int fpx_step_wait(fpx_engine* e, int32_t* n_out_p2b, int32_t* n_out_nack, int32_
   CK(e, cudaSetDevice(e->cfg.device));
   fpx_engine::Lane& ln = e->lane[e->lane_tail];
   CK(e, cudaEventSynchronize(ln.ev_done));
-  const DevStatus& st = *ln.h_st;
+  const DevStatus& st = *ln.h_st;   // copied behind the step's kernels by fpx_step_submit
   int status = FPX_OK;
-  if (st.err_word != ~0ull) {
-    status = -(int)(st.err_word & 0xff);
-    if (err_index) *err_index = (long long)(st.err_word >> 8);
-    unsigned long long none = ~0ull;   // the reference process would be dead; clear for the caller's fpx_reset
-    CK(e, cudaMemcpyAsync(&e->st->err_word, &none, 8, cudaMemcpyHostToDevice, e->stream));
-  }
+  const int c = take_error(e, st, e->st, e->stream, false, &status, err_index);
+  if (c != FPX_OK) return c;
   if (status == FPX_OK && st.n_chosen > 0)
     CK(e, cudaMemcpyAsync(ln.out_chosen, ln.d_out_chosen, (size_t)st.n_chosen * 8, cudaMemcpyDeviceToHost, e->d2h_stream));
   if (status == FPX_OK && st.n_nack > 0) {   // leader change in this batch: the dense copy is not the stream
@@ -907,8 +936,8 @@ int fpx_global_watermark_dev(fpx_engine* e, uint32_t epoch, int32_t timeout_ms, 
 }
 
 int fpx_step_arm_ms(fpx_engine* e, int32_t ring_slot, float* arm_ms) {
-  if (!e || !e->step_ev || ring_slot < 0 || !arm_ms) return FPX_ERR_INVALID_ARG;
-  cudaEvent_t* ev = e->step_ev + (size_t)(ring_slot % kStepRing) * 4;
+  if (!e || e->step_ev.empty() || ring_slot < 0 || !arm_ms) return FPX_ERR_INVALID_ARG;
+  cudaEvent_t* ev = e->step_ev.data() + (size_t)(ring_slot % kStepRing) * 4;
   CK(e, cudaEventSynchronize(ev[3]));
   CK(e, cudaEventElapsedTime(arm_ms, ev[1], ev[2]));
   return FPX_OK;
@@ -916,17 +945,10 @@ int fpx_step_arm_ms(fpx_engine* e, int32_t ring_slot, float* arm_ms) {
 
 int fpx_sync(fpx_engine* e, fpx_sync_result* out) {
   if (!e) return FPX_ERR_INVALID_ARG;
-  CK(e, cudaMemcpyAsync(e->h_st, e->st, sizeof(DevStatus), cudaMemcpyDeviceToHost, e->stream));
-  CK(e, cudaStreamSynchronize(e->stream));
   int status = FPX_OK;
-  long long idx = -1;
-  if (e->h_st->err_word != ~0ull) {
-    status = -(int)(e->h_st->err_word & 0xff);
-    idx = (long long)(e->h_st->err_word >> 8);
-    unsigned long long none = ~0ull;
-    CK(e, cudaMemcpyAsync(&e->st->err_word, &none, 8, cudaMemcpyHostToDevice, e->stream));
-    CK(e, cudaStreamSynchronize(e->stream));
-  }
+  int64_t idx = -1;
+  const int c = read_status(e, e->h_st, e->st, e->stream, &status, &idx);
+  if (c != FPX_OK) return c;
   if (out) {
     out->status = status;
     out->reserved = 0;
@@ -945,14 +967,8 @@ int fpx_proxyleader_arm(fpx_engine* e, const fpx_p2a* in, int32_t n, int64_t* er
   if (err_index) *err_index = -1;
   int c = check_n(e, in, n);
   if (c != FPX_OK || n == 0) return c;
-  CK(e, cudaSetDevice(e->cfg.device));
-  CK(e, cudaMemcpyAsync(e->d_in, in, (size_t)n * 16, cudaMemcpyHostToDevice, e->stream));
-  c = fpx_proxyleader_arm_dev(e, (const fpx_p2a*)e->d_in, n);
-  if (c != FPX_OK) return c;
-  fpx_sync_result r;
-  c = fpx_sync(e, &r);
-  if (err_index) *err_index = r.err_index;
-  return c;
+  return staged_call(e, in, (size_t)n * 16, err_index, nullptr,
+                     [&](void* d) { return fpx_proxyleader_arm_dev(e, (const fpx_p2a*)d, n); });
 }
 
 int fpx_acceptor_phase2a(fpx_engine* e, const fpx_p2a* in, int32_t n, fpx_p2b* out_p2b, int32_t* n_p2b,
@@ -1009,13 +1025,10 @@ int fpx_proxyleader_phase2b(fpx_engine* e, const fpx_p2b* in, int32_t n, fpx_cho
   int c = check_n(e, in, n);
   if (c != FPX_OK || n == 0) return c;
   if (!out || !n_out) return FPX_ERR_INVALID_ARG;
-  CK(e, cudaSetDevice(e->cfg.device));
-  CK(e, cudaMemcpyAsync(e->d_in, in, (size_t)n * 16, cudaMemcpyHostToDevice, e->stream));
-  c = fpx_proxyleader_phase2b_dev(e, (const fpx_p2b*)e->d_in, n, (fpx_chosen*)e->d_out_b);
-  if (c != FPX_OK) return c;
   fpx_sync_result r;
-  c = fpx_sync(e, &r);
-  if (err_index) *err_index = r.err_index;
+  c = staged_call(e, in, (size_t)n * 16, err_index, &r, [&](void* d) {
+    return fpx_proxyleader_phase2b_dev(e, (const fpx_p2b*)d, n, (fpx_chosen*)e->d_out_b);
+  });
   if (c != FPX_OK) return c;
   *n_out = r.n_chosen;
   if (r.n_chosen) {
@@ -1038,14 +1051,8 @@ int fpx_vm_client_request(fpx_engine* e, const fpx_p2a* in, int32_t n, int64_t* 
   int c = check_n(e, in, n);
   if (c != FPX_OK || n == 0) return c;
   if (e->g.protocol != FPX_VANILLA_MENCIUS) return FPX_ERR_UNSUPPORTED;
-  CK(e, cudaSetDevice(e->cfg.device));
-  CK(e, cudaMemcpyAsync(e->d_in, in, (size_t)n * 16, cudaMemcpyHostToDevice, e->stream));
-  c = fpx_vm_client_request_dev(e, (const fpx_p2a*)e->d_in, n);
-  if (c != FPX_OK) return c;
-  fpx_sync_result r;
-  c = fpx_sync(e, &r);
-  if (err_index) *err_index = r.err_index;
-  return c;
+  return staged_call(e, in, (size_t)n * 16, err_index, nullptr,
+                     [&](void* d) { return fpx_vm_client_request_dev(e, (const fpx_p2a*)d, n); });
 }
 
 // which: 0 handlePhase2a (d_reply dense), 1 handleChosen
@@ -1076,15 +1083,11 @@ static int vm_call(fpx_engine* e, const void* in, int32_t n, fpx_p2b* reply, int
   if (c != FPX_OK || n == 0) return c;
   if (e->g.protocol != FPX_VANILLA_MENCIUS) return FPX_ERR_UNSUPPORTED;
   if (which == 0 && !reply) return FPX_ERR_INVALID_ARG;
-  CK(e, cudaSetDevice(e->cfg.device));
-  CK(e, cudaMemcpyAsync(e->d_in, in, (size_t)n * 16, cudaMemcpyHostToDevice, e->stream));
-  c = vm_launch(e, e->d_in, n, (fpx_p2b*)e->d_out_a, which);
-  if (c != FPX_OK) return c;
-  if (which == 0) CK(e, cudaMemcpyAsync(reply, e->d_out_a, (size_t)n * 16, cudaMemcpyDeviceToHost, e->stream));
-  fpx_sync_result r;
-  c = fpx_sync(e, &r);
-  if (err_index) *err_index = r.err_index;
-  return c;
+  return staged_call(e, in, (size_t)n * 16, err_index, nullptr, [&](void* d) {
+    const int rc = vm_launch(e, d, n, (fpx_p2b*)e->d_out_a, which);
+    if (rc == FPX_OK && which == 0) CK(e, cudaMemcpyAsync(reply, e->d_out_a, (size_t)n * 16, cudaMemcpyDeviceToHost, e->stream));
+    return rc;
+  });
 }
 
 int fpx_vm_phase2a(fpx_engine* e, const fpx_p2a* in, int32_t n, fpx_p2b* reply, int64_t* err_index) {
@@ -1114,14 +1117,8 @@ int fpx_replica_chosen(fpx_engine* e, const fpx_chosen* in, int32_t n, int64_t* 
   if (err_index) *err_index = -1;
   int c = check_n(e, in, n);
   if (c != FPX_OK || n == 0) return c;
-  CK(e, cudaSetDevice(e->cfg.device));
-  CK(e, cudaMemcpyAsync(e->d_in, in, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
-  c = fpx_replica_chosen_dev(e, (const fpx_chosen*)e->d_in, n);
-  if (c != FPX_OK) return c;
-  fpx_sync_result r;
-  c = fpx_sync(e, &r);
-  if (err_index) *err_index = r.err_index;
-  return c;
+  return staged_call(e, in, (size_t)n * 8, err_index, nullptr,
+                     [&](void* d) { return fpx_replica_chosen_dev(e, (const fpx_chosen*)d, n); });
 }
 
 int fpx_chosen_watermark(fpx_engine* e, int32_t* out) {
@@ -1154,43 +1151,40 @@ int fpx_quorum_eval(fpx_engine* e, int32_t which, const uint32_t* masks, int32_t
   if (!e || which < 0 || which > 3 || n < 0 || (n > 0 && (!masks || !out))) return FPX_ERR_INVALID_ARG;
   if (n == 0) return FPX_OK;
   CK(e, cudaSetDevice(e->cfg.device));
+  CudaResources tmp(e->cfg.device);   // this call's temporaries
   uint32_t* d_m = nullptr;
   uint8_t* d_o = nullptr;
-  CK(e, cudaMalloc(&d_m, (size_t)n * 4));
-  CK(e, cudaMalloc(&d_o, (size_t)n));
+  CK(e, tmp.alloc(&d_m, (size_t)n * 4));
+  CK(e, tmp.alloc(&d_o, (size_t)n));
   CK(e, cudaMemcpyAsync(d_m, masks, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
   quorum_eval_kernel<<<(n + 255) / 256, 256, 0, e->stream>>>(e->g, which, d_m, n, d_o);
   e->launches++;
   CK(e, cudaMemcpyAsync(out, d_o, (size_t)n, cudaMemcpyDeviceToHost, e->stream));
   CK(e, cudaStreamSynchronize(e->stream));
-  cudaFree(d_m);
-  cudaFree(d_o);
   return FPX_OK;
 }
 
 int fpx_snapshot_acceptor(fpx_engine* e, int32_t group, int32_t acceptor, int32_t* round,
                           int32_t* max_voted_slot, int32_t first_slot, int32_t n_slots, int32_t* vote_round,
                           int32_t* vote_value) {
-  if (!e || group < 0 || group >= e->g.groups || acceptor < 0 || acceptor >= e->g.per_group || n_slots < 0)
+  if (!e || group < 0 || group >= e->g.groups || acceptor < 0 || acceptor >= e->g.per_group || n_slots < 0 ||
+      (n_slots > 0 && (!vote_round || !vote_value)))
     return FPX_ERR_INVALID_ARG;
   CK(e, cudaSetDevice(e->cfg.device));
+  CudaResources tmp(e->cfg.device);
   int key = group * e->g.per_group + acceptor;
   if (round) CK(e, cudaMemcpyAsync(round, e->acc_round + key, 4, cudaMemcpyDeviceToHost, e->stream));
   if (max_voted_slot)
     CK(e, cudaMemcpyAsync(max_voted_slot, e->acc_max_voted + key, 4, cudaMemcpyDeviceToHost, e->stream));
   if (n_slots > 0) {
-    if (!vote_round || !vote_value) return FPX_ERR_INVALID_ARG;
     int32_t *d_r = nullptr, *d_v = nullptr;
-    CK(e, cudaMalloc(&d_r, (size_t)n_slots * 4));
-    CK(e, cudaMalloc(&d_v, (size_t)n_slots * 4));
+    CK(e, tmp.alloc(&d_r, (size_t)n_slots * 4));
+    CK(e, tmp.alloc(&d_v, (size_t)n_slots * 4));
     snapshot_votes_kernel<<<(n_slots + 255) / 256, 256, 0, e->stream>>>(e->g, e->votes, group, acceptor,
                                                                          first_slot, n_slots, d_r, d_v);
     e->launches++;
     CK(e, cudaMemcpyAsync(vote_round, d_r, (size_t)n_slots * 4, cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaMemcpyAsync(vote_value, d_v, (size_t)n_slots * 4, cudaMemcpyDeviceToHost, e->stream));
-    CK(e, cudaStreamSynchronize(e->stream));
-    cudaFree(d_r);
-    cudaFree(d_v);
   }
   CK(e, cudaStreamSynchronize(e->stream));
   return FPX_OK;
@@ -1222,10 +1216,11 @@ int fpx_leader_safe_values(fpx_engine* e, uint32_t responders, int32_t first_slo
   *max_slot = -1;
   if (n_slots == 0) return FPX_OK;
   CK(e, cudaSetDevice(e->cfg.device));
+  CudaResources tmp(e->cfg.device);
   int32_t *d_r = nullptr, *d_v = nullptr, *d_m = nullptr;
-  CK(e, cudaMalloc(&d_r, (size_t)n_slots * 4));
-  CK(e, cudaMalloc(&d_v, (size_t)n_slots * 4));
-  CK(e, cudaMalloc(&d_m, 4));
+  CK(e, tmp.alloc(&d_r, (size_t)n_slots * 4));
+  CK(e, tmp.alloc(&d_v, (size_t)n_slots * 4));
+  CK(e, tmp.alloc(&d_m, 4));
   CK(e, cudaMemsetAsync(d_m, 0xff, 4, e->stream));
   safe_values_kernel<<<(n_slots + 255) / 256, 256, 0, e->stream>>>(e->g, e->votes, responders, first_slot, n_slots,
                                                                     d_r, d_v, d_m);
@@ -1234,7 +1229,6 @@ int fpx_leader_safe_values(fpx_engine* e, uint32_t responders, int32_t first_slo
   CK(e, cudaMemcpyAsync(value_id, d_v, (size_t)n_slots * 4, cudaMemcpyDeviceToHost, e->stream));
   CK(e, cudaMemcpyAsync(max_slot, d_m, 4, cudaMemcpyDeviceToHost, e->stream));
   CK(e, cudaStreamSynchronize(e->stream));
-  cudaFree(d_r); cudaFree(d_v); cudaFree(d_m);
   return FPX_OK;
 }
 
@@ -1242,13 +1236,13 @@ int fpx_snapshot_log(fpx_engine* e, int32_t first_slot, int32_t n_slots, int32_t
   if (!e || n_slots < 0 || (n_slots > 0 && !value_id)) return FPX_ERR_INVALID_ARG;
   if (n_slots == 0) return FPX_OK;
   CK(e, cudaSetDevice(e->cfg.device));
+  CudaResources tmp(e->cfg.device);
   int32_t* d_v = nullptr;
-  CK(e, cudaMalloc(&d_v, (size_t)n_slots * 4));
+  CK(e, tmp.alloc(&d_v, (size_t)n_slots * 4));
   snapshot_log_kernel<<<(n_slots + 255) / 256, 256, 0, e->stream>>>(e->g, e->rlog, first_slot, n_slots, d_v);
   e->launches++;
   CK(e, cudaMemcpyAsync(value_id, d_v, (size_t)n_slots * 4, cudaMemcpyDeviceToHost, e->stream));
   CK(e, cudaStreamSynchronize(e->stream));
-  cudaFree(d_v);
   return FPX_OK;
 }
 

@@ -272,6 +272,36 @@ def test_tally_dev_form_and_sync_counts():
     r.close(); eng.close()
 
 
+def test_engine_destroyed_first_with_work_queued():
+    """The engine goes first, with the reads handle's device-form batches still queued on its stream; then the
+    reads handle goes, and a new pair on the same device matches the oracle."""
+    import torch
+    cfg = RT.SHAPES["grid2x3"]
+    eng, r, ora = tally_pair(cfg, READS_CLIENT, 256, 4096)
+    trace = RT.tally_trace(12, cfg, READS_CLIENT, 256, 3, 4096)
+    dev = torch.device("cuda", 0)
+    queued = []
+    for op in trace:
+        if op[0] == "open":
+            r.open(op[1], op[2]); ora.open(op[1], op[2])
+            continue
+        d_in = torch.from_numpy(op[1].view(np.int32).reshape(-1, 4).copy()).to(dev)
+        d_out = torch.zeros((len(op[1]), 4), dtype=torch.int32, device=dev)
+        torch.cuda.synchronize()
+        r.max_slot_replies_dev(d_in.data_ptr(), len(op[1]), d_out.data_ptr())
+        queued.append((d_in, d_out, ora.max_slot_replies(op[1])[2]))
+    eng.close()   # drains the engine's stream: every queued batch has run
+    for _, d_out, want in queued:
+        got = d_out.cpu().numpy()
+        RT.same_outputs([got[:len(want)].reshape(-1).view(RO.READ_SLOT)], [want], "queued dev form")
+        assert not got[len(want):].any()
+    assert sum(len(w) for _, _, w in queued) > 0
+    r.close()
+    eng, r, ora = tally_pair(cfg, READS_CLIENT, 256, 4096)
+    RT.same_outputs(RT.run_tally(r, trace), RT.run_tally(ora, trace), "after the engine went first")
+    r.close(); eng.close()
+
+
 def test_create_checks():
     eng = engine(RT.SHAPES["cfg1"])
     with pytest.raises(FpxError) as ei:
