@@ -28,6 +28,9 @@ SYMBOLS = [
     "fpx_global_watermark", "fpx_global_watermark_dev",
     "fpx_conflict_index_create", "fpx_conflict_index_destroy", "fpx_conflict_index_put_snapshot", "fpx_conflict_index_batch",
     "fpx_depgraph_create", "fpx_depgraph_destroy", "fpx_depgraph_commit", "fpx_depgraph_update_executed", "fpx_depgraph_execute",
+    "fpx_epaxos_graph_create", "fpx_epaxos_graph_destroy", "fpx_epaxos_graph_commit", "fpx_epaxos_graph_commit_dev",
+    "fpx_epaxos_graph_sync", "fpx_epaxos_graph_stream", "fpx_epaxos_graph_update_executed", "fpx_epaxos_graph_execute",
+    "fpx_epaxos_graph_last_kernel_ms",
     "fpx_epaxos_stream", "fpx_epaxos_sync", "fpx_epaxos_lead_dev", "fpx_epaxos_preaccept_dev", "fpx_epaxos_accept_dev",
     "fpx_epaxos_preacceptok_dev", "fpx_epaxos_acceptok_dev", "fpx_epaxos_preaccept_sets",
     "fpx_epaxos_create", "fpx_epaxos_destroy", "fpx_epaxos_lead", "fpx_epaxos_preaccept", "fpx_epaxos_accept",

@@ -23,6 +23,7 @@
 #include "fpx_conflict.cuh"
 #include "fpx_depgraph.cuh"
 #include "fpx_epaxos.cuh"
+#include "fpx_epaxos_graph.cuh"
 #include "fpx_host.h"
 #include "fpx_ranges.cuh"
 #include "fpx_reads.cuh"

@@ -264,6 +264,15 @@ def _bind_f4(L):
     L.fpx_depgraph_commit.argtypes = [vp, vp, vp, vp, vp, i32, p(C.c_int64)]; L.fpx_depgraph_commit.restype = i32
     L.fpx_depgraph_update_executed.argtypes = [vp, vp, i32, p(C.c_int64)]; L.fpx_depgraph_update_executed.restype = i32
     L.fpx_depgraph_execute.argtypes = [vp, vp, vp, p(i32), vp]; L.fpx_depgraph_execute.restype = i32
+    L.fpx_epaxos_graph_create.argtypes = [p(vp), i32, i32, i32, i32]; L.fpx_epaxos_graph_create.restype = i32
+    L.fpx_epaxos_graph_destroy.argtypes = [vp]; L.fpx_epaxos_graph_destroy.restype = None
+    L.fpx_epaxos_graph_commit.argtypes = [vp, vp, i32, p(C.c_int64)]; L.fpx_epaxos_graph_commit.restype = i32
+    L.fpx_epaxos_graph_commit_dev.argtypes = [vp, vp, i32]; L.fpx_epaxos_graph_commit_dev.restype = i32
+    L.fpx_epaxos_graph_sync.argtypes = [vp, p(C.c_int64)]; L.fpx_epaxos_graph_sync.restype = i32
+    L.fpx_epaxos_graph_stream.argtypes = [vp]; L.fpx_epaxos_graph_stream.restype = vp
+    L.fpx_epaxos_graph_update_executed.argtypes = [vp, vp]; L.fpx_epaxos_graph_update_executed.restype = i32
+    L.fpx_epaxos_graph_execute.argtypes = [vp, vp, vp, p(i32), vp]; L.fpx_epaxos_graph_execute.restype = i32
+    L.fpx_epaxos_graph_last_kernel_ms.argtypes = [vp]; L.fpx_epaxos_graph_last_kernel_ms.restype = C.c_float
     L._f4_bound = True
 
 
@@ -367,3 +376,81 @@ class DependencyGraph:
                 comps.append([])
             comps[-1].append(int(out[p]))
         return comps, np.nonzero(bl)[0].tolist()
+
+
+class EpaxosGraph:
+    """TarjanDependencyGraph over EPaxos instances with dense InstancePrefixSet dependencies on the GPU
+    (include/fpx.h, fpx_epaxos_graph_*).  Commit rows are fpx_epaxos_commit's: {inst_replica, inst_number,
+    value_id, seq, deps[n]}; deps[inst_replica] > inst_number is the instance's own hole, not a dependency."""
+
+    def __init__(self, n_replicas, instances_per_replica, max_batch=1 << 16, device=0):
+        self._L = _lib.lib()
+        _bind_f4(self._L)
+        self.n, self.cap = n_replicas, instances_per_replica
+        self.h = C.c_void_p()
+        st = self._L.fpx_epaxos_graph_create(C.byref(self.h), n_replicas, instances_per_replica, max_batch, device)
+        if st != 0:
+            self.h = None
+            raise FpxError(st)
+
+    def close(self):
+        if getattr(self, "h", None):
+            self._L.fpx_epaxos_graph_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def commit(self, rows):
+        rows = np.ascontiguousarray(rows, dtype=np.int32).reshape(-1, 4 + self.n)
+        err = C.c_int64(-1)
+        st = self._L.fpx_epaxos_graph_commit(self.h, rows.ctypes.data, len(rows), C.byref(err))
+        if st != 0:
+            raise FpxError(st, err.value)
+
+    @property
+    def stream(self):
+        return self._L.fpx_epaxos_graph_stream(self.h)
+
+    def commit_dev(self, d_in, n):
+        """the same rows in device memory, asynchronous on self.stream; errors collected by sync()"""
+        st = self._L.fpx_epaxos_graph_commit_dev(self.h, d_in, n)
+        if st != 0:
+            raise FpxError(st)
+
+    def sync(self):
+        err = C.c_int64(-1)
+        st = self._L.fpx_epaxos_graph_sync(self.h, C.byref(err))
+        if st != 0:
+            raise FpxError(st, err.value)
+
+    def update_executed(self, watermark):
+        """updateExecuted of every instance (c, j < watermark[c])"""
+        wm = np.ascontiguousarray(watermark, dtype=np.int32)
+        st = self._L.fpx_epaxos_graph_update_executed(self.h, wm.ctypes.data)
+        if st != 0:
+            raise FpxError(st)
+
+    def execute_raw(self):
+        """(rows [m, 2] of {replica, number}, component heads [m], blockers [n, cap] as 0/1)"""
+        nv = self.n * self.cap
+        out = np.zeros((nv, 2), dtype=np.int32); head = np.zeros(nv, dtype=np.uint8)
+        bl = np.zeros((self.n, self.cap), dtype=np.uint8)
+        m = C.c_int32(0)
+        st = self._L.fpx_epaxos_graph_execute(self.h, out.ctypes.data, head.ctypes.data, C.byref(m), bl.ctypes.data)
+        if st != 0:
+            raise FpxError(st)
+        return out[:m.value], head[:m.value], bl
+
+    def execute_by_component(self):
+        """(components in dependency order, each a list of (replica, number) sorted by (seq, replica, number);
+        sorted blockers as (replica, number))"""
+        out, head, bl = self.execute_raw()
+        comps = []
+        for p in range(len(out)):
+            if head[p]:
+                comps.append([])
+            comps[-1].append((int(out[p, 0]), int(out[p, 1])))
+        return comps, [(int(c), int(j)) for c, j in zip(*np.nonzero(bl))]
+
+    def last_kernel_ms(self):
+        return float(self._L.fpx_epaxos_graph_last_kernel_ms(self.h))

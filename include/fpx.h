@@ -657,6 +657,36 @@ int fpx_depgraph_commit(fpx_depgraph* g, const int32_t* keys, const int32_t* seq
                         int32_t n, int64_t* err_index);
 int fpx_depgraph_update_executed(fpx_depgraph* g, const int32_t* keys, int32_t n, int64_t* err_index);
 int fpx_depgraph_execute(fpx_depgraph* g, int32_t* out_keys, uint8_t* out_component_head, int32_t* n_out, uint8_t* blockers);
+/* The same graph specialised to EPaxos instances with dense InstancePrefixSet dependencies (Replica.scala:864-886):
+ * instance (c, j), c < n_replicas <= 7, j < instances_per_replica, depends on every (c', j') with j' < deps[c'],
+ * except itself (subtractOne, Replica.scala:582): deps[c] > j is a hole, never a self-dependency.  No edge is
+ * materialised; execute runs in O(log(n * instances_per_replica)) launches (DESIGN §6b).
+ * commit: rows of 4+n ints, the layout of fpx_epaxos_commit's input: {inst_replica, inst_number, value_id (ignored),
+ * seq, deps[n]}.  An instance already committed or executed is ignored; within a batch the first record of an
+ * instance wins; an instance outside the handle is FPX_ERR_SLOT_RANGE at its record and nothing of the batch is
+ * applied.  A watermark above instances_per_replica names instances that can never be committed: the vertex is
+ * never executable.  commit_dev: the same rows in device memory, asynchronous on fpx_epaxos_graph_stream, the
+ * error collected by fpx_epaxos_graph_sync.
+ * update_executed: updateExecuted of every (c, j < watermark[c]).
+ * execute = executeByComponent(None): out rows {inst_replica, inst_number} of the executable instances, as
+ * strongly connected components in dependency order, each sorted by (seq, replica, number); out_component_head[p]
+ * = 1 where a component starts.  Components are ordered by (sum of the closure vector, ...) (DESIGN §6b).  out
+ * holds 2 * n * instances_per_replica ints, out_component_head n * instances_per_replica bytes.  blockers
+ * (optional, n * instances_per_replica bytes, index c * instances_per_replica + j): 1 for every absent instance
+ * that a committed, unexecuted instance names.  The executables are marked executed. */
+typedef struct fpx_epaxos_graph fpx_epaxos_graph;
+int fpx_epaxos_graph_create(fpx_epaxos_graph** out, int32_t n_replicas, int32_t instances_per_replica, int32_t max_batch,
+                            int32_t device);
+void fpx_epaxos_graph_destroy(fpx_epaxos_graph* g);
+int fpx_epaxos_graph_commit(fpx_epaxos_graph* g, const int32_t* in, int32_t n_rec, int64_t* err_index);
+int fpx_epaxos_graph_commit_dev(fpx_epaxos_graph* g, const int32_t* d_in, int32_t n_rec);
+int fpx_epaxos_graph_sync(fpx_epaxos_graph* g, int64_t* err_index);
+void* fpx_epaxos_graph_stream(fpx_epaxos_graph* g);
+int fpx_epaxos_graph_update_executed(fpx_epaxos_graph* g, const int32_t* watermark);
+int fpx_epaxos_graph_execute(fpx_epaxos_graph* g, int32_t* out, uint8_t* out_component_head, int32_t* n_out,
+                             uint8_t* blockers);
+/* device time (ms, CUDA events) of the kernels of the last commit or execute, without host round trips */
+float fpx_epaxos_graph_last_kernel_ms(fpx_epaxos_graph* g);
 
 /* One pipeline step from HOST buffers, asynchronous and double-buffered, for co-located roles on one GPU
  * (pinned host memory recommended).  fpx_step_submit enqueues: H2D of the Phase2a batch and of the Phase2b
