@@ -157,6 +157,12 @@ def lib():
         L.fpx_debug_set_acceptor_segments.argtypes = [vp, i32]; L.fpx_debug_set_acceptor_segments.restype = i32
     if hasattr(L, "fpx_debug_set_tally_max_sub"):
         L.fpx_debug_set_tally_max_sub.argtypes = [vp, i32]; L.fpx_debug_set_tally_max_sub.restype = i32
+    if hasattr(L, "fpx_debug_set_counters"):
+        u32 = C.c_uint32
+        L.fpx_debug_set_counters.argtypes = [vp, u32, u32, u32, u32]; L.fpx_debug_set_counters.restype = i32
+        L.fpx_debug_get_counters.argtypes = [vp, vp]; L.fpx_debug_get_counters.restype = i32
+        L.fpx_debug_epaxos_set_counters.argtypes = [vp, u32, u32]; L.fpx_debug_epaxos_set_counters.restype = i32
+        L.fpx_debug_epaxos_get_counters.argtypes = [vp, vp]; L.fpx_debug_epaxos_get_counters.restype = i32
     if L.fpx_abi_version() != 1:
         raise ImportError("libfpx.so ABI version mismatch")
     _lib = L

@@ -543,6 +543,25 @@ int fpx_debug_last_tally_path(fpx_engine* e) {
   CK(e, cudaMemcpy(&v, &e->st->ts_path, 4, cudaMemcpyDeviceToHost));
   return (int)v;
 }
+// Undocumented test aids: the host's 32-bit counters {seq_base (Phase2b stamps), rseq_base (Chosen log numbers),
+// rng_seq_base (Phase2bNoopRange stamps), vm_tag (vanilla Mencius batch tag)}, so that a test can start them just
+// below their wrap and run the renormalization and tag-reuse paths through real calls.  Host fields only: no
+// device memory is written.  Each value must lie in 1 .. 0xfffffffe, the range the counters themselves take.
+static bool counter_ok(uint32_t v) { return v != 0u && v != 0xffffffffu; }
+int fpx_debug_set_counters(fpx_engine* e, uint32_t seq_base, uint32_t rseq_base, uint32_t rng_seq_base, uint32_t vm_tag) {
+  if (!e || !counter_ok(seq_base) || !counter_ok(rseq_base) || !counter_ok(rng_seq_base) || !counter_ok(vm_tag))
+    return FPX_ERR_INVALID_ARG;
+  e->seq_base = seq_base;
+  e->rseq_base = rseq_base;
+  e->rng_seq_base = rng_seq_base;
+  e->vm_tag = vm_tag;
+  return FPX_OK;
+}
+int fpx_debug_get_counters(fpx_engine* e, uint32_t* out) {
+  if (!e || !out) return FPX_ERR_INVALID_ARG;
+  out[0] = e->seq_base; out[1] = e->rseq_base; out[2] = e->rng_seq_base; out[3] = e->vm_tag;
+  return FPX_OK;
+}
 
 // --------------------------------------------------------------------------- device entry points
 
@@ -1066,11 +1085,20 @@ static int vm_launch(fpx_engine* e, const void* d_in, int32_t n, fpx_p2b* d_repl
   P.g = e->g; P.in = (const int4*)d_in; P.out = (int4*)d_reply; P.n = n; P.votes = e->votes;
   P.rows = e->rows; P.st = e->st;
   P.tag = e->vm_tag++;
-  if (e->vm_tag == 0xffffffffu) e->vm_tag = 1;
   if (which == 0) vm_phase2a_kernel<<<std::min((n + 256 * kVmUnroll - 1) / (256 * kVmUnroll), e->num_sms * FPX_VM_CTAS_PER_SM), 256, 0, e->stream>>>(P);
   else vm_learn_chosen_kernel<<<(n + 255) / 256, 256, 0, e->stream>>>(P);
   e->launches++;
   CK(e, cudaGetLastError());
+  if (e->vm_tag == 0xffffffffu) {
+    // Every batch tag has been used: the next call reuses tag 1, and a cell still claimed by the call of that
+    // tag one cycle earlier would fail its Phase2a as a second claim of the batch.  Claims only mean something
+    // inside one batch: reset them all behind this call's kernel.  Once per 2^32 - 2 calls.
+    const size_t cells = (size_t)e->g.local_slots * e->g.voters;
+    vm_claim_init_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, e->stream>>>(e->votes, cells);
+    e->launches++;
+    CK(e, cudaGetLastError());
+    e->vm_tag = 1;
+  }
   return FPX_OK;
 }
 

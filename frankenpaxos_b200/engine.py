@@ -160,6 +160,23 @@ class Engine:
         """Cut every tally call into launches of at most `votes` votes (0: the default, 10,485,760)."""
         self._check(self._L.fpx_debug_set_tally_max_sub(self.h, votes))
 
+    COUNTERS = ("seq_base", "rseq_base", "rng_seq_base", "vm_tag")
+
+    def set_counters(self, **values):
+        """Start the host's 32-bit counters (COUNTERS; unnamed ones keep their value) anywhere in 1 .. 2**32 - 2,
+        e.g. just below their wrap."""
+        unknown = set(values) - set(self.COUNTERS)
+        if unknown:
+            raise ValueError(f"unknown counters {sorted(unknown)}")
+        cur = self.counters()
+        self._check(self._L.fpx_debug_set_counters(self.h, *(values.get(k, cur[k]) for k in self.COUNTERS)))
+
+    def counters(self):
+        """{name: value} of the host's 32-bit counters."""
+        out = np.zeros(4, dtype=np.uint32)
+        self._check(self._L.fpx_debug_get_counters(self.h, out.ctypes.data))
+        return dict(zip(self.COUNTERS, (int(x) for x in out)))
+
     @property
     def last_tally_path(self):
         """'sweep' / 'exact': what the last proxyleader_phase2b launch did."""

@@ -214,6 +214,23 @@ class EpaxosReplica:
             raise FpxError(st)
         return out, lk.value, lb
 
+    # -- test aids (not part of include/fpx.h)
+    def set_counters(self, tag=None, seq_base=None):
+        """Start the batch tag and the response stamp numbering anywhere in 1 .. 2**32 - 2 (None: unchanged)."""
+        cur = self.counters()
+        st = self._L.fpx_debug_epaxos_set_counters(self.h, cur["tag"] if tag is None else tag,
+                                                   cur["seq_base"] if seq_base is None else seq_base)
+        if st != 0:
+            raise FpxError(st)
+
+    def counters(self):
+        """{'tag': next batch tag, 'seq_base': next response stamp}"""
+        out = np.zeros(2, dtype=np.uint32)
+        st = self._L.fpx_debug_epaxos_get_counters(self.h, out.ctypes.data)
+        if st != 0:
+            raise FpxError(st)
+        return {"tag": int(out[0]), "seq_base": int(out[1])}
+
 
 def depset_union(watermarks, value_lists, group_off, device=0):
     """Batched IntPrefixSet union on the GPU.  watermarks[j], value_lists[j] (iterable of
