@@ -297,7 +297,7 @@ const char* fpx_strerror(int s) {
     case FPX_ERR_CONFLICT: return "too many same-key/different-value conflicts in one batch";
     case FPX_ERR_NO_DEVICE: return "no CUDA device";
     case FPX_ERR_UNSUPPORTED: return "configuration not supported by this engine build";
-    case FPX_ERR_BATCH_ORDER: return "EPaxos batch contract violated: split the batch at err_index";
+    case FPX_ERR_BATCH_ORDER: return "batch contract violated (fpx_epaxos_*: nothing applied, split the batch at err_index; vanilla Mencius Phase2a / Mencius range fill: half applied, fpx_reset)";
     case FPX_ERR_CHECK_FAILED: return "a logger.check of the reference failed";
     case FPX_ERR_WIRE: return "malformed protobuf message (InvalidProtocolBufferException)";
     case FPX_ERR_EXCHANGE_TIMEOUT: return "a shard of the log did not publish its watermark in time";

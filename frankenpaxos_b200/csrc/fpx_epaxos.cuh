@@ -4,8 +4,9 @@
 //   transitionToPreAcceptPhase :633-729, transitionToAcceptPhase :732-793, commit :815-829.
 //   S/epaxos/InstancePrefixSet.scala:121-126 -> S/compact/IntPrefixSet.scala:317-351 (dep-set union).
 //
-// One thread per message.  Batch contract (checked on the device, violations are
-// FPX_ERR_BATCH_ORDER with the offending index, never a wrong answer):
+// One thread per message.  Batch contract (checked on the device by a validation pass AHEAD of the
+// handler kernels: a violation is FPX_ERR_BATCH_ORDER with the index to split at and nothing of the
+// call is applied, never a wrong answer):
 //   E1  PreAccept / Accept / lead batches hold at most one message per instance;
 //   E2  PreAcceptOk / AcceptOk batches hold at most one message per (instance,
 //       replica); a response that REPLACES an earlier one with different content
@@ -53,10 +54,14 @@ struct EpGeometry {
 struct EpState {
   int32_t* cmd;                    // [n*per_replica][kEpCmdWords]
   int32_t* lead;                   // [n*per_replica][kEpLeadWords]
-  unsigned long long* claim;       // [n*per_replica]  (~batch_tag : min index) of the running batch
-  unsigned long long* count;       // [n*per_replica]  (batch_tag : #records) of the running batch
+  // scratch of the validation pass, tagged with the batch tag (a word of another tag is ignored)
+  unsigned long long* claim;       // [n*per_replica]  (~batch_tag : min index) over the batch's records of the instance
+  unsigned long long* rclaim;      // [n*per_replica][kEpMaxN]  the same per (instance, sender) of a response batch
+  uint32_t* refused;               // [0] batch tag of the call the validation pass refused, 0 = none; stays until the
+                                   //     status is collected.  [1] batch tag of the last call with a replacing response
   unsigned long long* largest;     // largestBallot as an order-preserving key
   unsigned long long* proc_ballot; // [max_batch] ballot key of record i if it "proceeded", else 0
+  int32_t* vflag;                  // [max_batch] validation of a response batch: 0 not counted, 1 counted, 2 replacing
   DevStatus* st;
 };
 
@@ -72,26 +77,24 @@ __device__ __forceinline__ long long ep_instance(const EpGeometry& g, int rep, i
   if ((uint32_t)rep >= (uint32_t)g.n || (uint32_t)num >= (uint32_t)g.per_replica) return -1;
   return (long long)num * g.n + rep;
 }
-// contract E1/E2: min index of this batch per instance; returns true if another
-// record of this batch already claimed the instance with a smaller/larger index
-__device__ __forceinline__ bool ep_claim(const EpState& s, long long inst, uint32_t tag, int i) {
-  unsigned long long mine = ((unsigned long long)(~tag) << 32) | (uint32_t)i;
-  unsigned long long old = atomicMin(&s.claim[inst], mine);
-  if ((uint32_t)(old >> 32) == ~tag) {
-    report_error(s.st, FPX_ERR_BATCH_ORDER, max((long long)i, (long long)(uint32_t)old));
-    return true;
-  }
-  return false;
+// min index of this batch per key (instance, or instance and sender); returns the index that held the key
+// before this one, -1 if none did
+__device__ __forceinline__ long long ep_claim(unsigned long long* word, uint32_t tag, int i) {
+  const unsigned long long mine = ((unsigned long long)(~tag) << 32) | (uint32_t)i;
+  const unsigned long long old = atomicMin(word, mine);
+  return (uint32_t)(old >> 32) == ~tag ? (long long)(uint32_t)old : -1;
 }
-__device__ __forceinline__ uint32_t ep_count(const EpState& s, long long inst, uint32_t tag) {
-  unsigned long long* p = &s.count[inst];
-  unsigned long long old = *p, assumed;
-  do {
-    assumed = old;
-    unsigned long long nw = ((uint32_t)(assumed >> 32) == tag) ? assumed + 1 : (((unsigned long long)tag << 32) | 1u);
-    old = atomicCAS(p, assumed, nw);
-  } while (old != assumed);
-  return 0;
+// A call refused by its validation pass applies nothing: its handler kernels return at entry, and so do the
+// kernels of every call queued behind it until the status has been collected (fpx_epaxos_sync).
+__device__ __forceinline__ bool ep_refused(const EpState& s) { return __ldcg(s.refused) != 0; }
+// the validation kernels of the calls queued behind a refused one return as well: the status is the refused call's
+__device__ __forceinline__ bool ep_refused_before(const EpState& s, uint32_t tag) {
+  const uint32_t r = __ldcg(s.refused);
+  return r != 0 && r != tag;
+}
+__device__ __forceinline__ void ep_refuse(const EpState& s, uint32_t tag, int code, long long index) {
+  report_error(s.st, code, index);
+  *(volatile uint32_t*)s.refused = tag;
 }
 
 struct EpParams {
@@ -124,6 +127,31 @@ __device__ __forceinline__ void ep_stage_rows(const int32_t* in, long long tile0
   for (int e = (words & ~3) + threadIdx.x; e < words; e += kEpTile) s_in[(e / W) * Wp + e % W] = in[tile0 * W + e];
 }
 
+// ---- The validation pass: one launch ahead of a call's handler kernels (two for PreAcceptOk / PrepareOk).  It
+// reads {rep, num[, ballot, from]} of every row and the state the call starts from, and writes nothing but scratch
+// tagged with the batch tag.  What it refuses -- an instance or sender out of range (FPX_ERR_SLOT_RANGE), a
+// prepare-phase ballot past FPX_MAX_ROUND (FPX_ERR_ROUND_RANGE), a batch that breaks E1 / E2
+// (FPX_ERR_BATCH_ORDER, the later index of the first colliding pair: both halves of a split there are smaller and
+// the first is legal) -- is refused whole: no handler kernel of the call runs.
+// E1 calls and handleNack (no contract, claims = false): rows of W words.
+__global__ void __launch_bounds__(kEpTile) ep_validate_kernel(EpParams P, int W, bool claims, bool prepare_phase) {
+  if (ep_refused_before(P.s, P.tag)) return;
+  const int i = blockIdx.x * kEpTile + threadIdx.x;
+  if (i >= P.n_rec) return;
+  const int32_t* r = P.in + (size_t)i * W;
+  const long long inst = ep_instance(P.g, r[0], r[1]);
+  if (inst < 0) { ep_refuse(P.s, P.tag, FPX_ERR_SLOT_RANGE, i); return; }
+  if (prepare_phase) {                                            // row i gets ordering L + 1 + i
+    int L, rep;
+    key_ballot(max(__ldcg(P.s.largest), ballot_key(0, P.g.index)), L, rep);
+    if ((long long)L + 1 + i > FPX_MAX_ROUND) { ep_refuse(P.s, P.tag, FPX_ERR_ROUND_RANGE, i); return; }
+  }
+  if (claims) {
+    const long long other = ep_claim(&P.s.claim[inst], P.tag, i);
+    if (other >= 0) ep_refuse(P.s, P.tag, FPX_ERR_BATCH_ORDER, max((long long)i, other));
+  }
+}
+
 // word w of a fresh leader row (transitionToPreAcceptPhase, :695-724): PreAccepting in the message's ballot, no
 // AcceptOk / PreAcceptOk stamps except the leader's own PreAcceptOk, which is "before everything" (:716-724)
 __device__ __forceinline__ int32_t ep_lead_word(const EpGeometry& g, const int32_t* r, int w) {
@@ -139,10 +167,11 @@ __device__ __forceinline__ int32_t ep_lead_word(const EpGeometry& g, const int32
 }
 
 // ---- transitionToPreAcceptPhase (:633-729).  in row: {rep, num, b_ord, b_rep, value, seq, avoid, pad, deps[n]}
-// Thread t judges message t of the tile (claim, cmdLog header as two 128-bit loads, cmdLog row written as four
+// Thread t judges message t of the tile (cmdLog header as two 128-bit loads, cmdLog row written as four
 // 128-bit words); the 384-byte leader rows are then written by whole warps, lane L the 16 bytes at word 4L:
 // one fully coalesced store instruction per row instead of ~40 scalar ones.
 __global__ void __launch_bounds__(kEpTile) ep_lead_kernel(EpParams P) {
+  if (ep_refused(P.s)) return;
   const EpGeometry& g = P.g;
   extern __shared__ int32_t s_ep[];
   __shared__ long long s_inst[kEpTile];
@@ -157,9 +186,7 @@ __global__ void __launch_bounds__(kEpTile) ep_lead_kernel(EpParams P) {
     const int32_t* r = s_ep + tid * Wp;
     const int i = (int)tile0 + tid;
     const long long inst = ep_instance(g, r[0], r[1]);
-    if (inst < 0) {
-      report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
-    } else if (!ep_claim(P.s, inst, P.tag, i)) {
+    if (inst >= 0) {                                              // always: the validation pass judged the range
       int4* c4 = (int4*)(P.s.cmd + inst * kEpCmdWords);
       const int4 h0 = __ldcg(c4), h1 = __ldcg(c4 + 1);          // {kind, value, bord, brep} {vbord, vbrep, seq, pad}
       const unsigned long long b = ballot_key(r[2], r[3]);
@@ -209,6 +236,7 @@ __host__ __device__ __forceinline__ int ep_in_words(const EpGeometry& g, bool ac
 
 template <bool kAccept>
 __global__ void __launch_bounds__(kEpTile) ep_acceptor_kernel(EpParams P) {
+  if (ep_refused(P.s)) return;
   const EpGeometry& g = P.g;
   extern __shared__ int32_t s_ep[];
   __shared__ unsigned long long s_big[kEpTile / 32];
@@ -243,9 +271,7 @@ __global__ void __launch_bounds__(kEpTile) ep_acceptor_kernel(EpParams P) {
     o[0] = REPLY_NONE; o[1] = -1; o[2] = -1; o[3] = 0;
     for (int k = 0; k < g.n; ++k) o[4 + k] = 0;
     const long long inst = ep_instance(g, r[0], r[1]);
-    if (inst < 0) {
-      report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
-    } else if (!ep_claim(P.s, inst, P.tag, i)) {
+    if (inst >= 0) {                                              // always: the validation pass judged the range
       int4* c4 = (int4*)(P.s.cmd + inst * kEpCmdWords);
       const int4 h0 = __ldcg(c4), h1 = __ldcg(c4 + 1);          // {kind, value, bord, brep} {vbord, vbrep, seq, pad}
       const unsigned long long b = ballot_key(r[2], r[3]);
@@ -404,8 +430,8 @@ __global__ void ep_renormalize_kernel(EpState s, size_t n_inst) {
 // ---- handlePreAcceptOk (:1291-1419) / handleAcceptOk (:1514-1565), stamp pass
 // in row preacceptok: {rep, num, b_ord, b_rep, from, seq, deps[n]};  acceptok: {rep, num, b_ord, b_rep, from, pad}
 // mode[i] (scratch): 0 inactive, 1 first delivery of its replica, 2 replacing response.
-// The tile's input rows are staged coalesced; per message: one 128-bit load of the leader header, the batch
-// count, one atomicMin on the replica's stamp word, and the answer {seq, deps} as two 128-bit words (one sector).
+// The tile's input rows are staged coalesced; per message: one 128-bit load of the leader header, one atomicMin
+// on the replica's stamp word, and the answer {seq, deps} as two 128-bit words (one sector).
 __device__ __forceinline__ void ep_load8(const int32_t* p, int (&v)[8]) {
   const int4 a = __ldcg((const int4*)p), b = __ldcg((const int4*)p + 1);
   v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
@@ -433,10 +459,71 @@ __host__ __device__ __forceinline__ int ep_resp_in_words(const EpGeometry& g) {
   return kWhich == kRespAcceptOk ? 6 : kWhich == kRespPrepareOk ? 9 : 6 + g.n;
 }
 
+// Validation of a response batch (E2).  Only a response the handler would count takes part: the row leads the
+// instance in the phase the response belongs to, in the response's ballot -- judged on the state the call starts
+// from, which is what the stamp pass sees.  First launch: at most one such response per (instance, sender); vflag[i]
+// = 1 counted, 2 counted and REPLACING (its sender's answer is already stored, with other content); the smallest
+// counted index per instance goes to `claim`.  Second launch, once every claim is in (a grid-wide order: it cannot
+// be the same launch): a replacing response must be the only counted one of its instance.  The pairs are
+// (replacing, any other counted) -- with m the instance's smallest counted index, a replacing record i > m reports
+// i, and when the replacing record IS m every other counted record reports itself: the minimum is the pair's
+// later index either way.
+template <int kWhich>
+__global__ void __launch_bounds__(kEpTile) ep_validate_responses_kernel(EpParams P) {
+  constexpr bool kAccept = kWhich == kRespAcceptOk, kPrepare = kWhich == kRespPrepareOk;
+  if (ep_refused_before(P.s, P.tag)) return;
+  const EpGeometry& g = P.g;
+  const int i = blockIdx.x * kEpTile + threadIdx.x;
+  if (i >= P.n_rec) return;
+  const int32_t* r = P.in + (size_t)i * ep_resp_in_words<kWhich>(g);
+  int flag = 0;
+  const long long inst = ep_instance(g, r[0], r[1]);
+  const int from = r[4];
+  if (inst < 0 || (uint32_t)from >= (uint32_t)g.n) {
+    ep_refuse(P.s, P.tag, FPX_ERR_SLOT_RANGE, i);
+  } else {
+    const int32_t* l = P.s.lead + inst * kEpLeadWords;
+    const int4 h = __ldcg((const int4*)l);                                      // {kind, value, bord, brep}
+    const bool leading = h.x == (kAccept ? LK_ACCEPTING : kPrepare ? LK_PREPARING : LK_PREACCEPTING);
+    if (leading && ballot_key(r[2], r[3]) == ballot_key(h.z, h.w)) {
+      flag = 1;
+      ep_claim(&P.s.claim[inst], P.tag, i);
+      const long long other = ep_claim(&P.s.rclaim[inst * kEpMaxN + from], P.tag, i);
+      if (other >= 0) {
+        ep_refuse(P.s, P.tag, FPX_ERR_BATCH_ORDER, max((long long)i, other));
+      } else if (!kAccept && (uint32_t)__ldcg(&l[L_RSTAMP + from]) != kStampEmpty) {
+        int v[8], have[8];
+        ep_answer_of<kWhich>(g, r, v);
+        ep_load8(l + L_RESP + from * kEpRespWords, have);
+        bool same = true;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) same = same && (k > g.n || have[k] == v[k]);
+        if (!same) {
+          flag = 2;
+          *(volatile uint32_t*)(P.s.refused + 1) = P.tag;                       // the second launch has work
+        }
+      }
+    }
+  }
+  P.s.vflag[i] = flag;
+}
+__global__ void __launch_bounds__(kEpTile) ep_validate_replace_kernel(EpParams P, int W) {
+  if (__ldcg(P.s.refused + 1) != P.tag || ep_refused_before(P.s, P.tag)) return;
+  const int i = blockIdx.x * kEpTile + threadIdx.x;
+  if (i >= P.n_rec) return;
+  const int flag = __ldcg(P.s.vflag + i);
+  if (flag == 0) return;
+  const int32_t* r = P.in + (size_t)i * W;
+  const long long inst = ep_instance(P.g, r[0], r[1]);
+  const uint32_t m = (uint32_t)__ldcg(&P.s.claim[inst]);                        // of this batch: record i claimed too
+  if (m != (uint32_t)i && (flag == 2 || __ldcg(P.s.vflag + m) == 2)) ep_refuse(P.s, P.tag, FPX_ERR_BATCH_ORDER, i);
+}
+
 // the leader kinds the three response handlers count for: PreAcceptOk (:1295-1315), AcceptOk (:1518-1535),
 // PrepareOk (:1763-1784)
 template <int kWhich>
 __global__ void __launch_bounds__(kEpTile) ep_response_stamp_kernel(EpParams P, int32_t* mode) {
+  if (ep_refused(P.s)) return;
   constexpr bool kAccept = kWhich == kRespAcceptOk, kPrepare = kWhich == kRespPrepareOk;
   const EpGeometry& g = P.g;
   extern __shared__ int32_t s_ep[];
@@ -451,16 +538,13 @@ __global__ void __launch_bounds__(kEpTile) ep_response_stamp_kernel(EpParams P, 
   const int32_t* r = s_ep + tid * Wp;
   int md = 0;
   const long long inst = ep_instance(g, r[0], r[1]);
-  if (inst < 0 || (uint32_t)r[4] >= (uint32_t)g.n) {
-    report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
-  } else {
+  if (inst >= 0 && (uint32_t)r[4] < (uint32_t)g.n) {               // always: the validation pass judged the range
     int32_t* l = P.s.lead + inst * kEpLeadWords;
     const int4 h = __ldcg((const int4*)l);                                      // {kind, value, bord, brep}
     const bool leading = h.x == (kAccept ? LK_ACCEPTING : kPrepare ? LK_PREPARING : LK_PREACCEPTING);
     if (kPrepare && leading && ballot_key(r[2], r[3]) > ballot_key(h.z, h.w))
       report_error(P.s.st, FPX_ERR_CHECK_FAILED, i);                            // logger.checkLt (:1792)
     if (leading && ballot_key(r[2], r[3]) == ballot_key(h.z, h.w)) {            // :1325-1335 / :1543-1552 / :1785
-      ep_count(P.s, inst, P.tag);
       const uint32_t seq = P.seq_base + (uint32_t)i;
       const uint32_t old = atomicMin((uint32_t*)&l[(kAccept ? L_ASTAMP : L_RSTAMP) + r[4]], seq);
       if (old == kStampEmpty) {                                 // responses(replicaIndex) = ok (:1340 / :1796), new key
@@ -470,9 +554,7 @@ __global__ void __launch_bounds__(kEpTile) ep_response_stamp_kernel(EpParams P, 
           ep_answer_of<kWhich>(g, r, v);
           ep_store8(l + L_RESP + r[4] * kEpRespWords, v);
         }
-      } else if (old >= P.seq_base) {                           // two responses of one replica in one batch (E2)
-        report_error(P.s.st, FPX_ERR_BATCH_ORDER, max((uint32_t)i, old - P.seq_base));
-      } else if (!kAccept) {
+      } else if (!kAccept && old < P.seq_base) {                // (a stamp of this batch: excluded by E2)
         int v[8], have[8];
         ep_answer_of<kWhich>(g, r, v);
         ep_load8(l + L_RESP + r[4] * kEpRespWords, have);
@@ -548,6 +630,7 @@ __device__ __forceinline__ int ep_prepare_decide(const EpGeometry& g, const int 
 // {kind, b_ord, b_rep, value}), staged in shared memory and stored coalesced.
 template <int kWhich>
 __global__ void __launch_bounds__(kEpTile) ep_response_decide_kernel(EpParams P, const int32_t* mode) {
+  if (ep_refused(P.s)) return;
   constexpr bool kAccept = kWhich == kRespAcceptOk, kPrepare = kWhich == kRespPrepareOk;
   const EpGeometry& g = P.g;
   extern __shared__ int32_t s_ep[];
@@ -571,16 +654,11 @@ __global__ void __launch_bounds__(kEpTile) ep_response_decide_kernel(EpParams P,
       int32_t* c = P.s.cmd + inst * kEpCmdWords;
       const uint32_t seq = P.seq_base + (uint32_t)i;
       if (md == 2) {
-        // a replacing response must be alone for its instance in the batch (E2); size unchanged: no
-        // threshold can be crossed
-        const unsigned long long cnt = __ldcg(&P.s.count[inst]);
-        if ((uint32_t)(cnt >> 32) == P.tag && (uint32_t)cnt > 1) {
-          report_error(P.s.st, FPX_ERR_BATCH_ORDER, i);
-        } else {
-          int v[8];
-          ep_answer_of<kWhich>(g, r, v);
-          ep_store8(l + L_RESP + r[4] * kEpRespWords, v);
-        }
+        // a replacing response is alone for its instance in the batch (E2, judged by the validation pass): no
+        // decision of this batch reads the answer it replaces; size unchanged: no threshold can be crossed
+        int v[8];
+        ep_answer_of<kWhich>(g, r, v);
+        ep_store8(l + L_RESP + r[4] * kEpRespWords, v);
       } else {
         int st[8];
         ep_load8(l + (kAccept ? L_ASTAMP : L_RSTAMP), st);
@@ -707,6 +785,7 @@ __device__ __forceinline__ void ep_cta_max(unsigned long long m, unsigned long l
 // ---- handleCommit (:1567-1575) -> commit (:815-831).  in row: {rep, num, value, seq, deps[n]}; no reply.
 // CommittedEntry(triple) whatever the entry held (:826-827) and no leader state of any kind (:831).
 __global__ void __launch_bounds__(kEpTile) ep_commit_kernel(EpParams P) {
+  if (ep_refused(P.s)) return;
   const EpGeometry& g = P.g;
   extern __shared__ int32_t s_ep[];
   const int W = 4 + g.n, Wp = W | 1;
@@ -716,12 +795,9 @@ __global__ void __launch_bounds__(kEpTile) ep_commit_kernel(EpParams P) {
   ep_stage_rows(P.in, tile0, rows, W, Wp, s_ep);
   __syncthreads();
   if (tid >= rows) return;
-  const int i = (int)tile0 + tid;
   const int32_t* r = s_ep + tid * Wp;
   const long long inst = ep_instance(g, r[0], r[1]);
-  if (inst < 0) {
-    report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
-  } else if (!ep_claim(P.s, inst, P.tag, i)) {
+  if (inst >= 0) {                                              // always: the validation pass judged the range
     int dd[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) dd[k] = k < g.n ? r[4 + k] : 0;
@@ -738,6 +814,7 @@ __global__ void __launch_bounds__(kEpTile) ep_commit_kernel(EpParams P) {
 // largestBallot (:1578; a max, so the batch order does not matter); RECOVER_TIMER when a leader state of any kind
 // has a ballot below the Nack's (:1580-1618), i.e. the caller (re)arms the recoverInstance timer (:1623-1629).
 __global__ void __launch_bounds__(kEpTile) ep_nack_kernel(EpParams P) {
+  if (ep_refused(P.s)) return;
   const EpGeometry& g = P.g;
   extern __shared__ int32_t s_ep[];
   const int W = 4, Wp = W | 1;
@@ -752,9 +829,7 @@ __global__ void __launch_bounds__(kEpTile) ep_nack_kernel(EpParams P) {
     const int32_t* r = s_ep + tid * Wp;
     int kind = EV_NONE;
     const long long inst = ep_instance(g, r[0], r[1]);
-    if (inst < 0) {
-      report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
-    } else {
+    if (inst >= 0) {                                              // always: the validation pass judged the range
       seen = ballot_key(r[2], r[3]);
       const int4 lh = __ldcg((const int4*)(P.s.lead + inst * kEpLeadWords));   // {kind, value, bord, brep}
       if (lh.x != LK_NONE && ballot_key(lh.z, lh.w) < seen) kind = EV_RECOVER_TIMER;
@@ -770,6 +845,7 @@ __global__ void __launch_bounds__(kEpTile) ep_nack_kernel(EpParams P) {
 // turn (:976).  The row's leader state becomes Preparing in that ballot with no responses (the replica's own
 // PrepareOk arrives as a message, :985); cmdLog is not touched.
 __global__ void __launch_bounds__(kEpTile) ep_prepare_phase_kernel(EpParams P) {
+  if (ep_refused(P.s)) return;
   const EpGeometry& g = P.g;
   const int i = blockIdx.x * kEpTile + threadIdx.x;
   int L, rep;
@@ -780,11 +856,7 @@ __global__ void __launch_bounds__(kEpTile) ep_prepare_phase_kernel(EpParams P) {
     const long long ord = (long long)L + 1 + i;
     int2 out = make_int2(-1, -1);
     const long long inst = ep_instance(g, r.x, r.y);
-    if (inst < 0) {
-      report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
-    } else if (ord > FPX_MAX_ROUND) {
-      report_error(P.s.st, FPX_ERR_ROUND_RANGE, i);
-    } else if (!ep_claim(P.s, inst, P.tag, i)) {
+    if (inst >= 0 && ord <= FPX_MAX_ROUND) {                      // always: the validation pass judged both
       int4* l4 = (int4*)(P.s.lead + inst * kEpLeadWords);
       const int4 empty = make_int4((int)kStampEmpty, (int)kStampEmpty, (int)kStampEmpty, (int)kStampEmpty);
       __stcg(l4, make_int4(LK_PREPARING, 0, (int)ord, g.index));
@@ -804,6 +876,7 @@ __global__ void __launch_bounds__(kEpTile) ep_prepare_phase_kernel(EpParams P) {
 // b = the Prepare's ballot), Nack (kind NACK, b = largestBallot, filled by the fix-up pass), Commit (kind COMMIT,
 // the triple).  Fields a reply does not carry are (-1, -1) ballots and zeros.
 __global__ void __launch_bounds__(kEpTile) ep_prepare_kernel(EpParams P) {
+  if (ep_refused(P.s)) return;
   const EpGeometry& g = P.g;
   extern __shared__ int32_t s_ep[];
   const int W = 4, Wp = W | 1, WO = 9 + g.n, WOp = WO | 1;
@@ -821,9 +894,7 @@ __global__ void __launch_bounds__(kEpTile) ep_prepare_kernel(EpParams P) {
     o[0] = REPLY_NONE; o[1] = 0; o[2] = -1; o[3] = -1; o[4] = -1; o[5] = -1; o[6] = ST_NOT_SEEN; o[7] = 0; o[8] = 0;
     for (int k = 0; k < g.n; ++k) o[9 + k] = 0;
     const long long inst = ep_instance(g, r[0], r[1]);
-    if (inst < 0) {
-      report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
-    } else if (!ep_claim(P.s, inst, P.tag, i)) {
+    if (inst >= 0) {                                              // always: the validation pass judged the range
       const unsigned long long b = ballot_key(r[2], r[3]);
       seen = b;                                                 // largestBallot = max(.., prepare.ballot) (:1637)
       int32_t* l = P.s.lead + inst * kEpLeadWords;
@@ -873,6 +944,7 @@ __global__ void __launch_bounds__(kEpTile) ep_prepare_kernel(EpParams P) {
 // the timer armed (LF_TIMER, set where EV_TIMER was emitted) takes the slow path, over every answer it holds; in
 // any other state the reference's stopTimers (:618-630) has cancelled the timer and the event is NONE.
 __global__ void __launch_bounds__(kEpTile) ep_slow_path_timer_kernel(EpParams P) {
+  if (ep_refused(P.s)) return;
   const EpGeometry& g = P.g;
   extern __shared__ int32_t s_ep[];
   const int W = 4, Wp = W | 1, WO = 2 + g.n;                    // odd: conflict-free as it is
@@ -883,14 +955,11 @@ __global__ void __launch_bounds__(kEpTile) ep_slow_path_timer_kernel(EpParams P)
   ep_stage_rows(P.in, tile0, rows, W, Wp, s_ep);
   __syncthreads();
   if (tid < rows) {
-    const int i = (int)tile0 + tid;
     const int32_t* r = s_ep + tid * Wp;
     int32_t* o = s_out + tid * WO;
     for (int k = 0; k < WO; ++k) o[k] = 0;                      // o[0] = EV_NONE
     const long long inst = ep_instance(g, r[0], r[1]);
-    if (inst < 0) {
-      report_error(P.s.st, FPX_ERR_SLOT_RANGE, i);
-    } else if (!ep_claim(P.s, inst, P.tag, i)) {
+    if (inst >= 0) {                                              // always: the validation pass judged the range
       int32_t* l = P.s.lead + inst * kEpLeadWords;
       int32_t* c = P.s.cmd + inst * kEpCmdWords;
       const int4 h0 = __ldcg((const int4*)l);                   // {kind, value, bord, brep}

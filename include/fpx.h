@@ -98,9 +98,13 @@ typedef enum {
                                       the in-batch order could not be resolved exactly   */
   FPX_ERR_NO_DEVICE = -10,
   FPX_ERR_UNSUPPORTED = -11,
-  FPX_ERR_BATCH_ORDER = -12,       /* EPaxos batch contract E1/E2 violated (two messages of
-                                      one instance / one (instance, replica) in one call):
-                                      split the batch at err_index and resubmit           */
+  FPX_ERR_BATCH_ORDER = -12,       /* fpx_epaxos_*: batch contract E1/E2 violated (two messages
+                                      of one instance / one (instance, replica) in one call).
+                                      NOTHING of the call is applied (outputs unspecified):
+                                      resubmit rows [0, err_index) and [err_index, n) as two
+                                      calls.  fpx_vm_phase2a, fpx_mencius_replica_chosen_range:
+                                      their batch contract violated; the call is HALF APPLIED,
+                                      fatal like every other status (fpx_reset)           */
   FPX_ERR_CHECK_FAILED = -14,      /* a logger.check of the reference failed (vanilla Mencius
                                       advanceWithSkips: a slot to skip is not vacant)   */
   FPX_ERR_WIRE = -15,              /* malformed protobuf bytes: what parseFrom rejects with
@@ -276,7 +280,9 @@ int fpx_leader_safe_values(fpx_engine* e, uint32_t responders, int32_t first_slo
  * and the coordinators' `phase2s`.  Skips, revocation and Phase 1 are control
  * path and out of scope (SURVEY.md 8(a) row a9).  Batch contract (checked, ->
  * FPX_ERR_BATCH_ORDER): at most one Phase2a per (slot, server) per call, because
- * the round compare is per log entry (:1016-1042), not per acceptor.          */
+ * the round compare is per log entry (:1016-1042), not per acceptor.  The key is
+ * in the message, so a caller can always flush ahead of a repeat; a call that
+ * returns the status is half applied and fatal like every other (fpx_reset).  */
 
 /* Server.handleClientRequest, state part (:767-829): the coordinator in.dst (which
  * must own in.slot) votes for its own command -- log(slot) = PendingEntry(0, 0,
@@ -354,7 +360,7 @@ int fpx_mencius_range_phase2b(fpx_engine* e, const fpx_p2b_range* in, int32_t n,
 /* Replica.handleChosenNoopRange (S/mencius/Replica.scala:464-486): slots start, start+LG,
  * ... < end are put as Noop UNTIL THE FIRST ONE ALREADY IN THE LOG, where the reference's
  * handler returns (:476-480).  Batch contract (FPX_ERR_BATCH_ORDER): two records of one
- * call must not cover a common slot.  With shard_count > 1 "already in the log" is judged
+ * call must not cover a common slot (the call is then half applied: fatal, fpx_reset).  With shard_count > 1 "already in the log" is judged
  * on this shard's slots only (use the _first / _fill pair below for the reference's result).  fpx_chosen_watermark afterwards is the first hole, i.e.
  * where executeLog stops when it next runs. */
 int fpx_mencius_replica_chosen_range(fpx_engine* e, const fpx_chosen_range* in, int32_t n, int64_t* err_index);
@@ -429,11 +435,20 @@ int fpx_wire_encode_chosen(fpx_engine* e, const fpx_chosen* in, int32_t n, const
  * sets go through fpx_depset_union.  Ballot = (ordering, replicaIndex), tuple
  * order (S/epaxos/BallotHelpers.scala:11-21).  Replies / events are DENSE: row i
  * of the output belongs to message i of the input (kind 0 = nothing to send).
- * Batch contract, checked on the device (FPX_ERR_BATCH_ORDER + first index):
- *   E1 lead / preaccept / accept: at most one message per instance per call;
- *   E2 preacceptok / acceptok: at most one message per (instance, replica) per
- *      call; a PreAcceptOk that replaces an earlier response of its replica with
- *      DIFFERENT content must be the only message of its instance in the call.
+ * Batch contract, checked on the device AHEAD of the handlers (FPX_ERR_BATCH_ORDER):
+ *   E1 lead / preaccept / accept / commit / prepare_phase / prepare /
+ *      slow_path_timer: at most one message per instance per call;
+ *   E2 preacceptok / acceptok / prepareok: at most one message per (instance,
+ *      replica) per call; a PreAcceptOk / PrepareOk that replaces an earlier response
+ *      of its replica with DIFFERENT content must be the only message of its instance
+ *      in the call.  (Only responses the handler counts take part: the instance is
+ *      led in that phase, in the response's ballot.)
+ * A batch in any order is legal for the reference, so this status is not fatal: a
+ * call that returns it -- or FPX_ERR_SLOT_RANGE / FPX_ERR_ROUND_RANGE -- has applied
+ * NOTHING (cmdLog, leader states and largestBallot are as before the call; its
+ * outputs are unspecified).  err_index is the later message of the first colliding
+ * pair: resubmit rows [0, err_index) and [err_index, n) as two calls (the second may
+ * be refused again, further in).  This guarantee holds for fpx_epaxos_* only.
  * What the conflict index would compute (computeSequenceNumberAndDependencies,
  * :569-600) is an INPUT: `local_deps` of a PreAccept, `deps` of lead.        */
 typedef struct fpx_epaxos fpx_epaxos;
@@ -479,7 +494,9 @@ int fpx_epaxos_preacceptok(fpx_epaxos* e, const int32_t* in, int32_t n_rec, int3
  * inst_number, ballot_ord, ballot_rep, from_replica, 0}; event rows as above (COMMIT). */
 int fpx_epaxos_acceptok(fpx_epaxos* e, const int32_t* in, int32_t n_rec, int32_t* event, int64_t* err_index);
 /* The same handlers on DEVICE-resident rows, asynchronous on the handle's stream (fpx_epaxos_stream, a
- * cudaStream_t); status and first offending index are collected by fpx_epaxos_sync. */
+ * cudaStream_t); status and first offending index are collected by fpx_epaxos_sync.  A refusal (see the batch
+ * contract above) stands until it is collected: the calls queued behind the refused one apply nothing either,
+ * fpx_epaxos_sync reports the refused call's status and index, and the caller resubmits all of them. */
 void* fpx_epaxos_stream(fpx_epaxos* e);
 int fpx_epaxos_sync(fpx_epaxos* e, int64_t* err_index);
 int fpx_epaxos_lead_dev(fpx_epaxos* e, const int32_t* d_in, int32_t n_rec);

@@ -1,7 +1,7 @@
 """BASELINE cfg4 (EPaxos, 5 replicas, 20 % conflicts, 2^20 instances) as seen by replica 0: device time of
 each handler batch on DEVICE-resident rows (fpx_epaxos_*_dev, CUDA events on the handle's stream, best of 3
 fresh replicas), with the algorithmic bytes per message next to it.
-Commit (the batch replica 0 receives for the instances it PreAccepted): 838 860 messages in 0.145 ms = 5.8 x 10^9
+Commit (the batch replica 0 receives for the instances it PreAccepted): 838 860 messages in 0.161 ms = 5.2 x 10^9
 messages/s, measured on an H100 80GB HBM3 at a 700 W power limit.
     python profiles/bench_epaxos_cfg4.py"""
 import json
