@@ -21,6 +21,7 @@
 #include "fpx_arm.cuh"
 #include "fpx_common.cuh"
 #include "fpx_conflict.cuh"
+#include "fpx_debug.h"
 #include "fpx_depgraph.cuh"
 #include "fpx_epaxos.cuh"
 #include "fpx_epaxos_graph.cuh"

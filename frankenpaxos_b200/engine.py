@@ -42,18 +42,57 @@ class FpxError(RuntimeError):
         super().__init__(f"fpx status {status} ({msg}) at record {index}{(': ' + detail) if detail else ''}")
 
 
+class _Handle:
+    """One handle of the C ABI: `create(&h, *args)` in the constructor (FpxError if it fails), `destroy(h)` on
+    close(), at the end of a `with` block, or when the object is collected."""
+
+    def __init__(self, create, destroy, *args):
+        self._L = _lib.lib()
+        self._destroy = getattr(self._L, destroy)
+        self.h = C.c_void_p()
+        st = getattr(self._L, create)(C.byref(self.h), *args)
+        if st != OK:
+            self.h = None
+            raise FpxError(st)
+
+    def close(self):
+        if getattr(self, "h", None):
+            self._destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def _check(self, st, idx=-1):
+        if st != OK:
+            raise FpxError(st, idx)
+
+    def _host_call(self, fn, *args):
+        """fn(h, *args, &err_index), a host-pointer form: FpxError at the record it reports."""
+        err = C.c_int64(-1)
+        self._check(fn(self.h, *args, C.byref(err)), err.value)
+
+
 def dst(group, acceptor):
     """fpx_p2a.dst encoding."""
     return (np.asarray(group, dtype=np.int32) << 16) | np.asarray(acceptor, dtype=np.int32)
 
 
-class Engine:
+class Engine(_Handle):
     """One GPU-resident {acceptors, proxy leader, replica log} for one config."""
 
     def __init__(self, f, num_acceptor_groups, acceptors_per_group, flexible=False, num_leaders=None,
                  num_replicas=None, slot_capacity=1 << 20, overflow_capacity=1 << 14, max_batch=1 << 20,
                  device=0, shard_index=0, shard_count=1, protocol=MULTIPAXOS, num_leader_groups=0):
-        L = _lib.lib()
         cfg = _lib.Config()
         cfg.struct_size = C.sizeof(_lib.Config)
         cfg.protocol = protocol
@@ -70,31 +109,9 @@ class Engine:
         cfg.shard_index, cfg.shard_count = shard_index, shard_count
         cfg.num_leader_groups = num_leader_groups
         self.cfg = cfg
-        self._L = L
-        self.h = C.c_void_p()
-        st = L.fpx_create(C.byref(self.h), C.byref(cfg))
-        if st != OK:
-            self.h = None
-            raise FpxError(st)
+        super().__init__("fpx_create", "fpx_destroy", C.byref(cfg))
 
     # -- life cycle
-    def close(self):
-        if getattr(self, "h", None):
-            self._L.fpx_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
-
     def reset(self):
         self._check(self._L.fpx_reset(self.h))
 
@@ -185,36 +202,29 @@ class Engine:
     # -- host-pointer calls (numpy in / numpy out)
     def proxyleader_arm(self, p2a):
         p2a = np.ascontiguousarray(p2a, dtype=P2A)
-        err = C.c_int64(-1)
-        st = self._L.fpx_proxyleader_arm(self.h, p2a.ctypes.data, len(p2a), C.byref(err))
-        self._check(st, err.value)
+        self._host_call(self._L.fpx_proxyleader_arm, p2a.ctypes.data, len(p2a))
 
     def acceptor_phase2a(self, p2a):
         p2a = np.ascontiguousarray(p2a, dtype=P2A)
         n = len(p2a)
         out = np.empty(max(n, 1), dtype=P2B)
         nack = np.empty(max(n, 1), dtype=NACK)
-        n1, n2, err = C.c_int32(0), C.c_int32(0), C.c_int64(-1)
-        st = self._L.fpx_acceptor_phase2a(self.h, p2a.ctypes.data, n, out.ctypes.data, C.byref(n1),
-                                          nack.ctypes.data, C.byref(n2), C.byref(err))
-        self._check(st, err.value)
+        n1, n2 = C.c_int32(0), C.c_int32(0)
+        self._host_call(self._L.fpx_acceptor_phase2a, p2a.ctypes.data, n, out.ctypes.data, C.byref(n1),
+                        nack.ctypes.data, C.byref(n2))
         return out[:n1.value], nack[:n2.value]
 
     def proxyleader_phase2b(self, p2b):
         p2b = np.ascontiguousarray(p2b, dtype=P2B)
         n = len(p2b)
         out = np.empty(max(n, 1), dtype=CHOSEN)
-        n1, err = C.c_int32(0), C.c_int64(-1)
-        st = self._L.fpx_proxyleader_phase2b(self.h, p2b.ctypes.data, n, out.ctypes.data, C.byref(n1),
-                                             C.byref(err))
-        self._check(st, err.value)
+        n1 = C.c_int32(0)
+        self._host_call(self._L.fpx_proxyleader_phase2b, p2b.ctypes.data, n, out.ctypes.data, C.byref(n1))
         return out[:n1.value]
 
     def replica_chosen(self, chosen):
         chosen = np.ascontiguousarray(chosen, dtype=CHOSEN)
-        err = C.c_int64(-1)
-        st = self._L.fpx_replica_chosen(self.h, chosen.ctypes.data, len(chosen), C.byref(err))
-        self._check(st, err.value)
+        self._host_call(self._L.fpx_replica_chosen, chosen.ctypes.data, len(chosen))
 
     def chosen_watermark(self):
         out = C.c_int32(0)
@@ -263,59 +273,51 @@ class Engine:
     # -- vanilla Mencius (protocol=VANILLA_MENCIUS)
     def vm_client_request(self, p2a):
         p2a = np.ascontiguousarray(p2a, dtype=P2A)
-        err = C.c_int64(-1)
-        self._check(self._L.fpx_vm_client_request(self.h, p2a.ctypes.data, len(p2a), C.byref(err)), err.value)
+        self._host_call(self._L.fpx_vm_client_request, p2a.ctypes.data, len(p2a))
 
     def vm_phase2a(self, p2a):
         """dense replies {group = kind (0 Phase2b, 1 Phase2Nack, 2 Chosen, 3 Chosen of a retired slot whose value
         is the shared log's executed entry), acceptor = server, slot, round|value (0 for kind 3)}"""
         p2a = np.ascontiguousarray(p2a, dtype=P2A)
         out = np.empty(max(len(p2a), 1), dtype=P2B)
-        err = C.c_int64(-1)
-        self._check(self._L.fpx_vm_phase2a(self.h, p2a.ctypes.data, len(p2a), out.ctypes.data, C.byref(err)), err.value)
+        self._host_call(self._L.fpx_vm_phase2a, p2a.ctypes.data, len(p2a), out.ctypes.data)
         return out[:len(p2a)]
 
     def vm_learn_chosen(self, recs):
         recs = np.ascontiguousarray(recs, dtype=P2B)
-        err = C.c_int64(-1)
-        self._check(self._L.fpx_vm_learn_chosen(self.h, recs.ctypes.data, len(recs), C.byref(err)), err.value)
+        self._host_call(self._L.fpx_vm_learn_chosen, recs.ctypes.data, len(recs))
 
     def vm_skip(self, recs):
         """Server.advanceWithSkips' log fill (own=1) / Server.handleSkip (own=0)."""
         recs = np.ascontiguousarray(recs, dtype=VM_SKIP)
-        err = C.c_int64(-1)
-        self._check(self._L.fpx_vm_skip(self.h, recs.ctypes.data, len(recs), C.byref(err)), err.value)
+        self._host_call(self._L.fpx_vm_skip, recs.ctypes.data, len(recs))
 
     # -- S/mencius Phase2aNoopRange path
     def mencius_arm_range(self, recs):
         recs = np.ascontiguousarray(recs, dtype=P2A_RANGE)
-        err = C.c_int64(-1)
-        self._check(self._L.fpx_mencius_arm_range(self.h, recs.ctypes.data, len(recs), C.byref(err)), err.value)
+        self._host_call(self._L.fpx_mencius_arm_range, recs.ctypes.data, len(recs))
 
     def mencius_acceptor_noop_range(self, recs):
         recs = np.ascontiguousarray(recs, dtype=P2A_RANGE)
         n = len(recs)
         out = np.zeros(max(n, 1), dtype=P2B_RANGE)
         nack = np.zeros(max(n, 1), dtype=NACK)
-        n1, n2, err = C.c_int32(0), C.c_int32(0), C.c_int64(-1)
-        self._check(self._L.fpx_mencius_acceptor_noop_range(self.h, recs.ctypes.data, n, out.ctypes.data, C.byref(n1),
-                                                            nack.ctypes.data, C.byref(n2), C.byref(err)), err.value)
+        n1, n2 = C.c_int32(0), C.c_int32(0)
+        self._host_call(self._L.fpx_mencius_acceptor_noop_range, recs.ctypes.data, n, out.ctypes.data, C.byref(n1),
+                        nack.ctypes.data, C.byref(n2))
         return out[:n1.value].copy(), nack[:n2.value].copy()
 
     def mencius_range_phase2b(self, recs):
         recs = np.ascontiguousarray(recs, dtype=P2B_RANGE)
         n = len(recs)
         out = np.zeros(max(n, 1), dtype=CHOSEN_RANGE)
-        n1, err = C.c_int32(0), C.c_int64(-1)
-        self._check(self._L.fpx_mencius_range_phase2b(self.h, recs.ctypes.data, n, out.ctypes.data, C.byref(n1),
-                                                      C.byref(err)), err.value)
+        n1 = C.c_int32(0)
+        self._host_call(self._L.fpx_mencius_range_phase2b, recs.ctypes.data, n, out.ctypes.data, C.byref(n1))
         return out[:n1.value].copy()
 
     def mencius_replica_chosen_range(self, recs):
         recs = np.ascontiguousarray(recs, dtype=CHOSEN_RANGE)
-        err = C.c_int64(-1)
-        self._check(self._L.fpx_mencius_replica_chosen_range(self.h, recs.ctypes.data, len(recs), C.byref(err)),
-                    err.value)
+        self._host_call(self._L.fpx_mencius_replica_chosen_range, recs.ctypes.data, len(recs))
 
     RANGE_NO_HIT = 0x7f7f7f7f
 
@@ -323,9 +325,7 @@ class Engine:
         """Per record: this shard's first slot of the range that is already in its log (RANGE_NO_HIT if none)."""
         recs = np.ascontiguousarray(recs, dtype=CHOSEN_RANGE)
         first = np.full(max(len(recs), 1), self.RANGE_NO_HIT, dtype=np.int32)
-        err = C.c_int64(-1)
-        self._check(self._L.fpx_mencius_replica_range_first(self.h, recs.ctypes.data, len(recs), first.ctypes.data,
-                                                            C.byref(err)), err.value)
+        self._host_call(self._L.fpx_mencius_replica_range_first, recs.ctypes.data, len(recs), first.ctypes.data)
         return first[:len(recs)]
 
     def mencius_replica_range_fill(self, recs, first):
@@ -333,9 +333,7 @@ class Engine:
         recs = np.ascontiguousarray(recs, dtype=CHOSEN_RANGE)
         first = np.ascontiguousarray(first, dtype=np.int32)
         assert len(first) == len(recs)
-        err = C.c_int64(-1)
-        self._check(self._L.fpx_mencius_replica_range_fill(self.h, recs.ctypes.data, len(recs), first.ctypes.data,
-                                                           C.byref(err)), err.value)
+        self._host_call(self._L.fpx_mencius_replica_range_fill, recs.ctypes.data, len(recs), first.ctypes.data)
 
     # -- wire codec: protobuf bytes of a batch of messages <-> records (include/fpx.h)
     def wire_decode_inbound(self, inbound, buf, offsets):
@@ -345,10 +343,8 @@ class Engine:
         n = len(offsets) - 1
         kind = np.zeros(max(n, 1), dtype=np.int32)
         rec = np.zeros(max(n, 1), dtype=WIRE_REC)
-        err = C.c_int64(-1)
-        self._check(self._L.fpx_wire_decode_inbound(self.h, inbound, buf.ctypes.data if len(buf) else None,
-                                                    offsets.ctypes.data, n, kind.ctypes.data, rec.ctypes.data,
-                                                    C.byref(err)), err.value)
+        self._host_call(self._L.fpx_wire_decode_inbound, inbound, buf.ctypes.data if len(buf) else None,
+                        offsets.ctypes.data, n, kind.ctypes.data, rec.ctypes.data)
         return kind[:n], rec[:n]
 
     def _wire_encode(self, fn, recs, dtype, max_per, *extra):
@@ -357,10 +353,7 @@ class Engine:
         cap = max(16, n * max_per) if not extra else extra[-1]
         out = np.zeros(cap, dtype=np.uint8)
         offs = np.zeros(n + 1, dtype=np.int32)
-        err = C.c_int64(-1)
-        args = [self.h, recs.ctypes.data, n] + list(extra[:-1] if extra else []) + [out.ctypes.data, cap, offs.ctypes.data,
-                                                                                     C.byref(err)]
-        self._check(fn(*args), err.value)
+        self._host_call(fn, recs.ctypes.data, n, *extra[:-1], out.ctypes.data, cap, offs.ctypes.data)
         return out[:offs[n]].copy(), offs
 
     def wire_encode_phase2b(self, recs):
@@ -428,9 +421,8 @@ class Engine:
 
     def step_wait(self):
         """Completes the oldest submitted step: (n_p2b, n_nack, n_chosen, watermark)."""
-        a, b, c, w, err = C.c_int32(0), C.c_int32(0), C.c_int32(0), C.c_int32(0), C.c_int64(-1)
-        st = self._L.fpx_step_wait(self.h, C.byref(a), C.byref(b), C.byref(c), C.byref(w), C.byref(err))
-        self._check(st, err.value)
+        a, b, c, w = C.c_int32(0), C.c_int32(0), C.c_int32(0), C.c_int32(0)
+        self._host_call(self._L.fpx_step_wait, C.byref(a), C.byref(b), C.byref(c), C.byref(w))
         return a.value, b.value, c.value, w.value
 
     def step_kernel_ms(self, ring_slot):

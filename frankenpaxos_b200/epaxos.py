@@ -6,7 +6,8 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .engine import FpxError
+from ._lib import EpaxosConfig
+from .engine import FpxError, _Handle
 
 REPLY_NONE, REPLY_OK, REPLY_NACK, REPLY_COMMIT = 0, 1, 2, 3
 EV_NONE, EV_FAST_COMMIT, EV_SLOW_ACCEPT, EV_TIMER, EV_COMMIT = 0, 1, 2, 3, 4
@@ -17,78 +18,16 @@ STATUS_NOT_SEEN, STATUS_PRE_ACCEPTED, STATUS_ACCEPTED = 0, 1, 2
 VALUE_NOOP = -(1 << 31)
 
 
-class EpaxosConfig(C.Structure):
-    _fields_ = [(n, C.c_int32) for n in ("struct_size", "f", "replica_index", "instances_per_replica",
-                                         "max_batch", "device")]
-
-
-def _bind(L):
-    if getattr(L, "_ep_bound", False):
-        return
-    vp, i32, p = C.c_void_p, C.c_int32, C.POINTER
-    L.fpx_epaxos_create.argtypes = [p(vp), p(EpaxosConfig)]; L.fpx_epaxos_create.restype = i32
-    L.fpx_epaxos_destroy.argtypes = [vp]; L.fpx_epaxos_destroy.restype = None
-    L.fpx_epaxos_lead.argtypes = [vp, vp, i32, p(C.c_int64)]; L.fpx_epaxos_lead.restype = i32
-    for nm in ("fpx_epaxos_preaccept", "fpx_epaxos_accept", "fpx_epaxos_preacceptok", "fpx_epaxos_acceptok"):
-        f = getattr(L, nm)
-        f.argtypes = [vp, vp, i32, vp, p(C.c_int64)]; f.restype = i32
-    L.fpx_epaxos_entry.argtypes = [vp, i32, i32, vp, p(i32), vp]; L.fpx_epaxos_entry.restype = i32
-    L.fpx_depset_union.argtypes = [i32, vp, vp, vp, i32, vp, i32, vp, vp, vp]; L.fpx_depset_union.restype = i32
-    L.fpx_epaxos_last_kernel_ms.argtypes = [vp]; L.fpx_epaxos_last_kernel_ms.restype = C.c_float
-    L.fpx_depset_union_dense_dev.argtypes = [i32, vp, i32, i32, i32, vp, vp]; L.fpx_depset_union_dense_dev.restype = i32
-    L.fpx_epaxos_stream.argtypes = [vp]; L.fpx_epaxos_stream.restype = vp
-    L.fpx_epaxos_sync.argtypes = [vp, p(C.c_int64)]; L.fpx_epaxos_sync.restype = i32
-    L.fpx_epaxos_lead_dev.argtypes = [vp, vp, i32]; L.fpx_epaxos_lead_dev.restype = i32
-    for nm in ("fpx_epaxos_preaccept_dev", "fpx_epaxos_accept_dev", "fpx_epaxos_preacceptok_dev", "fpx_epaxos_acceptok_dev"):
-        f = getattr(L, nm)
-        f.argtypes = [vp, vp, i32, vp]; f.restype = i32
-    L.fpx_epaxos_preaccept_sets.argtypes = [vp, vp, i32, vp, vp, p(C.c_int64)]; L.fpx_epaxos_preaccept_sets.restype = i32
-    L.fpx_epaxos_commit.argtypes = [vp, vp, i32, p(C.c_int64)]; L.fpx_epaxos_commit.restype = i32
-    for nm in ("fpx_epaxos_nack", "fpx_epaxos_prepare_phase", "fpx_epaxos_prepare", "fpx_epaxos_prepareok",
-               "fpx_epaxos_slow_path_timer"):
-        f = getattr(L, nm)
-        f.argtypes = [vp, vp, i32, vp, p(C.c_int64)]; f.restype = i32
-    L.fpx_epaxos_commit_dev.argtypes = [vp, vp, i32]; L.fpx_epaxos_commit_dev.restype = i32
-    for nm in ("fpx_epaxos_nack_dev", "fpx_epaxos_prepare_phase_dev", "fpx_epaxos_prepare_dev",
-               "fpx_epaxos_prepareok_dev", "fpx_epaxos_slow_path_timer_dev"):
-        f = getattr(L, nm)
-        f.argtypes = [vp, vp, i32, vp]; f.restype = i32
-    L._ep_bound = True
-
-
-class EpaxosReplica:
+class EpaxosReplica(_Handle):
     def __init__(self, f, replica_index, instances_per_replica, max_batch=1 << 16, device=0):
-        self._L = _lib.lib()
-        _bind(self._L)
         cfg = EpaxosConfig(C.sizeof(EpaxosConfig), f, replica_index, instances_per_replica, max_batch, device)
         self.f, self.n, self.index = f, 2 * f + 1, replica_index
-        self.h = C.c_void_p()
-        st = self._L.fpx_epaxos_create(C.byref(self.h), C.byref(cfg))
-        if st != 0:
-            self.h = None
-            raise FpxError(st)
-
-    def close(self):
-        if getattr(self, "h", None):
-            self._L.fpx_epaxos_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        super().__init__("fpx_epaxos_create", "fpx_epaxos_destroy", C.byref(cfg))
 
     def _call(self, fn, rows, width, out_width):
         rows = np.ascontiguousarray(rows, dtype=np.int32).reshape(-1, width)
         out = np.zeros((max(len(rows), 1), max(out_width, 1)), dtype=np.int32)
-        err = C.c_int64(-1)
-        if out_width:
-            st = fn(self.h, rows.ctypes.data, len(rows), out.ctypes.data, C.byref(err))
-        else:
-            st = fn(self.h, rows.ctypes.data, len(rows), C.byref(err))
-        if st != 0:
-            raise FpxError(st, err.value)
+        self._host_call(fn, rows.ctypes.data, len(rows), *((out.ctypes.data,) if out_width else ()))
         return out[:len(rows)]
 
     def lead(self, rows):
@@ -146,52 +85,40 @@ class EpaxosReplica:
         return self._L.fpx_epaxos_stream(self.h)
 
     def sync(self):
-        err = C.c_int64(-1)
-        st = self._L.fpx_epaxos_sync(self.h, C.byref(err))
-        if st != 0:
-            raise FpxError(st, err.value)
+        self._host_call(self._L.fpx_epaxos_sync)
 
     def lead_dev(self, d_in, n):
-        st = self._L.fpx_epaxos_lead_dev(self.h, d_in, n)
-        if st != 0:
-            raise FpxError(st)
-
-    def _dev(self, fn, d_in, n, d_out):
-        st = fn(self.h, d_in, n, d_out)
-        if st != 0:
-            raise FpxError(st)
+        self._check(self._L.fpx_epaxos_lead_dev(self.h, d_in, n))
 
     def preaccept_dev(self, d_in, n, d_reply):
-        self._dev(self._L.fpx_epaxos_preaccept_dev, d_in, n, d_reply)
+        self._check(self._L.fpx_epaxos_preaccept_dev(self.h, d_in, n, d_reply))
 
     def accept_dev(self, d_in, n, d_reply):
-        self._dev(self._L.fpx_epaxos_accept_dev, d_in, n, d_reply)
+        self._check(self._L.fpx_epaxos_accept_dev(self.h, d_in, n, d_reply))
 
     def preacceptok_dev(self, d_in, n, d_event):
-        self._dev(self._L.fpx_epaxos_preacceptok_dev, d_in, n, d_event)
+        self._check(self._L.fpx_epaxos_preacceptok_dev(self.h, d_in, n, d_event))
 
     def acceptok_dev(self, d_in, n, d_event):
-        self._dev(self._L.fpx_epaxos_acceptok_dev, d_in, n, d_event)
+        self._check(self._L.fpx_epaxos_acceptok_dev(self.h, d_in, n, d_event))
 
     def commit_dev(self, d_in, n):
-        st = self._L.fpx_epaxos_commit_dev(self.h, d_in, n)
-        if st != 0:
-            raise FpxError(st)
+        self._check(self._L.fpx_epaxos_commit_dev(self.h, d_in, n))
 
     def nack_dev(self, d_in, n, d_event):
-        self._dev(self._L.fpx_epaxos_nack_dev, d_in, n, d_event)
+        self._check(self._L.fpx_epaxos_nack_dev(self.h, d_in, n, d_event))
 
     def prepare_phase_dev(self, d_in, n, d_ballot):
-        self._dev(self._L.fpx_epaxos_prepare_phase_dev, d_in, n, d_ballot)
+        self._check(self._L.fpx_epaxos_prepare_phase_dev(self.h, d_in, n, d_ballot))
 
     def prepare_dev(self, d_in, n, d_reply):
-        self._dev(self._L.fpx_epaxos_prepare_dev, d_in, n, d_reply)
+        self._check(self._L.fpx_epaxos_prepare_dev(self.h, d_in, n, d_reply))
 
     def prepareok_dev(self, d_in, n, d_event):
-        self._dev(self._L.fpx_epaxos_prepareok_dev, d_in, n, d_event)
+        self._check(self._L.fpx_epaxos_prepareok_dev(self.h, d_in, n, d_event))
 
     def slow_path_timer_dev(self, d_in, n, d_event):
-        self._dev(self._L.fpx_epaxos_slow_path_timer_dev, d_in, n, d_event)
+        self._check(self._L.fpx_epaxos_slow_path_timer_dev(self.h, d_in, n, d_event))
 
     def preaccept_sets(self, rows, overflow_count):
         """handlePreAccept for possibly sparse sets: FPX_ERR_UNSUPPORTED at the first message that carries
@@ -199,36 +126,27 @@ class EpaxosReplica:
         rows = np.ascontiguousarray(rows, dtype=np.int32).reshape(-1, 6 + 2 * self.n)
         oc = np.ascontiguousarray(overflow_count, dtype=np.int32)
         out = np.zeros((max(len(rows), 1), 4 + self.n), dtype=np.int32)
-        err = C.c_int64(-1)
-        st = self._L.fpx_epaxos_preaccept_sets(self.h, rows.ctypes.data, len(rows), oc.ctypes.data, out.ctypes.data, C.byref(err))
-        if st != 0:
-            raise FpxError(st, err.value)
+        self._host_call(self._L.fpx_epaxos_preaccept_sets, rows.ctypes.data, len(rows), oc.ctypes.data, out.ctypes.data)
         return out[:len(rows)]
 
     def entry(self, rep, num):
         out = np.zeros(7 + self.n, dtype=np.int32)
         lk = C.c_int32(0)
         lb = np.zeros(2, dtype=np.int32)
-        st = self._L.fpx_epaxos_entry(self.h, rep, num, out.ctypes.data, C.byref(lk), lb.ctypes.data)
-        if st != 0:
-            raise FpxError(st)
+        self._check(self._L.fpx_epaxos_entry(self.h, rep, num, out.ctypes.data, C.byref(lk), lb.ctypes.data))
         return out, lk.value, lb
 
     # -- test aids (not part of include/fpx.h)
     def set_counters(self, tag=None, seq_base=None):
         """Start the batch tag and the response stamp numbering anywhere in 1 .. 2**32 - 2 (None: unchanged)."""
         cur = self.counters()
-        st = self._L.fpx_debug_epaxos_set_counters(self.h, cur["tag"] if tag is None else tag,
-                                                   cur["seq_base"] if seq_base is None else seq_base)
-        if st != 0:
-            raise FpxError(st)
+        self._check(self._L.fpx_debug_epaxos_set_counters(self.h, cur["tag"] if tag is None else tag,
+                                                          cur["seq_base"] if seq_base is None else seq_base))
 
     def counters(self):
         """{'tag': next batch tag, 'seq_base': next response stamp}"""
         out = np.zeros(2, dtype=np.uint32)
-        st = self._L.fpx_debug_epaxos_get_counters(self.h, out.ctypes.data)
-        if st != 0:
-            raise FpxError(st)
+        self._check(self._L.fpx_debug_epaxos_get_counters(self.h, out.ctypes.data))
         return {"tag": int(out[0]), "seq_base": int(out[1])}
 
 
@@ -237,7 +155,6 @@ def depset_union(watermarks, value_lists, group_off, device=0):
     ints > watermark); group q unions sets group_off[q]..group_off[q+1].  Returns a list of
     (watermark, sorted values)."""
     L = _lib.lib()
-    _bind(L)
     wm = np.ascontiguousarray(watermarks, dtype=np.int32)
     off = np.zeros(len(wm) + 1, dtype=np.int32)
     off[1:] = np.cumsum([len(v) for v in value_lists])
@@ -260,64 +177,23 @@ def depset_union(watermarks, value_lists, group_off, device=0):
 def depset_union_dense_dev(d_in, n_groups, sets_per_group, n_replicas, d_out, stream=None, device=0):
     """Dense batched union on device pointers: out[q][k] = max_r in[q][r][k] (asynchronous)."""
     L = _lib.lib()
-    _bind(L)
     st = L.fpx_depset_union_dense_dev(device, d_in, n_groups, sets_per_group, n_replicas, d_out, stream)
     if st != 0:
         raise FpxError(st)
 
 
 # --------------------------------------------------------------------------- execution side (SURVEY 8(f) rank 4)
-def _bind_f4(L):
-    if getattr(L, "_f4_bound", False):
-        return
-    vp, i32, p = C.c_void_p, C.c_int32, C.POINTER
-    L.fpx_conflict_index_create.argtypes = [p(vp), i32, i32, i32, i32, i32]; L.fpx_conflict_index_create.restype = i32
-    L.fpx_conflict_index_destroy.argtypes = [vp]; L.fpx_conflict_index_destroy.restype = None
-    L.fpx_conflict_index_put_snapshot.argtypes = [vp, i32, i32]; L.fpx_conflict_index_put_snapshot.restype = i32
-    L.fpx_conflict_index_batch.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, vp, p(C.c_int64)]
-    L.fpx_conflict_index_batch.restype = i32
-    L.fpx_depgraph_create.argtypes = [p(vp), i32, i32, i32, i32]; L.fpx_depgraph_create.restype = i32
-    L.fpx_depgraph_destroy.argtypes = [vp]; L.fpx_depgraph_destroy.restype = None
-    L.fpx_depgraph_commit.argtypes = [vp, vp, vp, vp, vp, i32, p(C.c_int64)]; L.fpx_depgraph_commit.restype = i32
-    L.fpx_depgraph_update_executed.argtypes = [vp, vp, i32, p(C.c_int64)]; L.fpx_depgraph_update_executed.restype = i32
-    L.fpx_depgraph_execute.argtypes = [vp, vp, vp, p(i32), vp]; L.fpx_depgraph_execute.restype = i32
-    L.fpx_epaxos_graph_create.argtypes = [p(vp), i32, i32, i32, i32]; L.fpx_epaxos_graph_create.restype = i32
-    L.fpx_epaxos_graph_destroy.argtypes = [vp]; L.fpx_epaxos_graph_destroy.restype = None
-    L.fpx_epaxos_graph_commit.argtypes = [vp, vp, i32, p(C.c_int64)]; L.fpx_epaxos_graph_commit.restype = i32
-    L.fpx_epaxos_graph_commit_dev.argtypes = [vp, vp, i32]; L.fpx_epaxos_graph_commit_dev.restype = i32
-    L.fpx_epaxos_graph_sync.argtypes = [vp, p(C.c_int64)]; L.fpx_epaxos_graph_sync.restype = i32
-    L.fpx_epaxos_graph_stream.argtypes = [vp]; L.fpx_epaxos_graph_stream.restype = vp
-    L.fpx_epaxos_graph_update_executed.argtypes = [vp, vp]; L.fpx_epaxos_graph_update_executed.restype = i32
-    L.fpx_epaxos_graph_execute.argtypes = [vp, vp, vp, p(i32), vp]; L.fpx_epaxos_graph_execute.restype = i32
-    L.fpx_epaxos_graph_last_kernel_ms.argtypes = [vp]; L.fpx_epaxos_graph_last_kernel_ms.restype = C.c_float
-    L._f4_bound = True
-
-
-class ConflictIndex:
+class ConflictIndex(_Handle):
     """KeyValueStore's top-1 conflict index on the GPU (include/fpx.h, fpx_conflict_index_*)."""
     QUERY_THEN_PUT, PUT, QUERY = 0, 1, 2
 
     def __init__(self, num_leaders, key_capacity=1 << 16, max_commands=1 << 16, max_keys=1 << 17, device=0):
-        self._L = _lib.lib()
-        _bind_f4(self._L)
         self.n = num_leaders
-        self.h = C.c_void_p()
-        st = self._L.fpx_conflict_index_create(C.byref(self.h), num_leaders, key_capacity, max_commands, max_keys, device)
-        if st != 0:
-            self.h = None
-            raise FpxError(st)
-
-    def close(self):
-        if getattr(self, "h", None):
-            self._L.fpx_conflict_index_destroy(self.h)
-            self.h = None
-
-    __del__ = close
+        super().__init__("fpx_conflict_index_create", "fpx_conflict_index_destroy", num_leaders, key_capacity,
+                         max_commands, max_keys, device)
 
     def put_snapshot(self, leader, id_):
-        st = self._L.fpx_conflict_index_put_snapshot(self.h, leader, id_)
-        if st != 0:
-            raise FpxError(st)
+        self._check(self._L.fpx_conflict_index_put_snapshot(self.h, leader, id_))
 
     def batch(self, leader, id_, is_set, key_lists, mode=0):
         """Commands in delivery order; key_lists[i] = the keys of command i.  Returns deps [n_cmd, num_leaders]
@@ -330,34 +206,18 @@ class ConflictIndex:
         keys = np.ascontiguousarray(np.concatenate([np.asarray(k, dtype=np.int32) for k in key_lists])
                                     if off[-1] else np.zeros(0, dtype=np.int32), dtype=np.int32)
         out = np.zeros((max(n, 1), self.n), dtype=np.int32)
-        err = C.c_int64(-1)
-        st = self._L.fpx_conflict_index_batch(self.h, leader.ctypes.data, id_.ctypes.data, is_set.ctypes.data,
-                                              off.ctypes.data, keys.ctypes.data if len(keys) else None, n, mode,
-                                              out.ctypes.data, C.byref(err))
-        if st != 0:
-            raise FpxError(st, err.value)
+        self._host_call(self._L.fpx_conflict_index_batch, leader.ctypes.data, id_.ctypes.data, is_set.ctypes.data,
+                        off.ctypes.data, keys.ctypes.data if len(keys) else None, n, mode, out.ctypes.data)
         return None if mode == self.PUT else out[:n]
 
 
-class DependencyGraph:
+class DependencyGraph(_Handle):
     """TarjanDependencyGraph on the GPU (include/fpx.h, fpx_depgraph_*): int keys in [0, key_capacity)."""
 
     def __init__(self, key_capacity=1 << 12, dep_pool_capacity=1 << 16, max_batch=1 << 12, device=0):
-        self._L = _lib.lib()
-        _bind_f4(self._L)
         self.cap = key_capacity
-        self.h = C.c_void_p()
-        st = self._L.fpx_depgraph_create(C.byref(self.h), key_capacity, dep_pool_capacity, max_batch, device)
-        if st != 0:
-            self.h = None
-            raise FpxError(st)
-
-    def close(self):
-        if getattr(self, "h", None):
-            self._L.fpx_depgraph_destroy(self.h)
-            self.h = None
-
-    __del__ = close
+        super().__init__("fpx_depgraph_create", "fpx_depgraph_destroy", key_capacity, dep_pool_capacity, max_batch,
+                         device)
 
     def commit(self, keys, seqs, dep_lists):
         n = len(keys)
@@ -366,27 +226,19 @@ class DependencyGraph:
         off[1:] = np.cumsum([len(d) for d in dep_lists])
         deps = np.ascontiguousarray(np.concatenate([np.asarray(d, dtype=np.int32) for d in dep_lists])
                                     if off[-1] else np.zeros(0, dtype=np.int32), dtype=np.int32)
-        err = C.c_int64(-1)
-        st = self._L.fpx_depgraph_commit(self.h, keys.ctypes.data, seqs.ctypes.data, off.ctypes.data,
-                                         deps.ctypes.data if len(deps) else None, n, C.byref(err))
-        if st != 0:
-            raise FpxError(st, err.value)
+        self._host_call(self._L.fpx_depgraph_commit, keys.ctypes.data, seqs.ctypes.data, off.ctypes.data,
+                        deps.ctypes.data if len(deps) else None, n)
 
     def update_executed(self, keys):
         keys = np.ascontiguousarray(keys, dtype=np.int32)
-        err = C.c_int64(-1)
-        st = self._L.fpx_depgraph_update_executed(self.h, keys.ctypes.data, len(keys), C.byref(err))
-        if st != 0:
-            raise FpxError(st, err.value)
+        self._host_call(self._L.fpx_depgraph_update_executed, keys.ctypes.data, len(keys))
 
     def execute_by_component(self):
         """(components in dependency order, each a list of keys sorted by (seq, key); sorted blockers)."""
         out = np.zeros(self.cap, dtype=np.int32); head = np.zeros(self.cap, dtype=np.uint8)
         bl = np.zeros(self.cap, dtype=np.uint8)
         n = C.c_int32(0)
-        st = self._L.fpx_depgraph_execute(self.h, out.ctypes.data, head.ctypes.data, C.byref(n), bl.ctypes.data)
-        if st != 0:
-            raise FpxError(st)
+        self._check(self._L.fpx_depgraph_execute(self.h, out.ctypes.data, head.ctypes.data, C.byref(n), bl.ctypes.data))
         comps = []
         for p in range(n.value):
             if head[p]:
@@ -395,34 +247,19 @@ class DependencyGraph:
         return comps, np.nonzero(bl)[0].tolist()
 
 
-class EpaxosGraph:
+class EpaxosGraph(_Handle):
     """TarjanDependencyGraph over EPaxos instances with dense InstancePrefixSet dependencies on the GPU
     (include/fpx.h, fpx_epaxos_graph_*).  Commit rows are fpx_epaxos_commit's: {inst_replica, inst_number,
     value_id, seq, deps[n]}; deps[inst_replica] > inst_number is the instance's own hole, not a dependency."""
 
     def __init__(self, n_replicas, instances_per_replica, max_batch=1 << 16, device=0):
-        self._L = _lib.lib()
-        _bind_f4(self._L)
         self.n, self.cap = n_replicas, instances_per_replica
-        self.h = C.c_void_p()
-        st = self._L.fpx_epaxos_graph_create(C.byref(self.h), n_replicas, instances_per_replica, max_batch, device)
-        if st != 0:
-            self.h = None
-            raise FpxError(st)
-
-    def close(self):
-        if getattr(self, "h", None):
-            self._L.fpx_epaxos_graph_destroy(self.h)
-            self.h = None
-
-    __del__ = close
+        super().__init__("fpx_epaxos_graph_create", "fpx_epaxos_graph_destroy", n_replicas, instances_per_replica,
+                         max_batch, device)
 
     def commit(self, rows):
         rows = np.ascontiguousarray(rows, dtype=np.int32).reshape(-1, 4 + self.n)
-        err = C.c_int64(-1)
-        st = self._L.fpx_epaxos_graph_commit(self.h, rows.ctypes.data, len(rows), C.byref(err))
-        if st != 0:
-            raise FpxError(st, err.value)
+        self._host_call(self._L.fpx_epaxos_graph_commit, rows.ctypes.data, len(rows))
 
     @property
     def stream(self):
@@ -430,22 +267,15 @@ class EpaxosGraph:
 
     def commit_dev(self, d_in, n):
         """the same rows in device memory, asynchronous on self.stream; errors collected by sync()"""
-        st = self._L.fpx_epaxos_graph_commit_dev(self.h, d_in, n)
-        if st != 0:
-            raise FpxError(st)
+        self._check(self._L.fpx_epaxos_graph_commit_dev(self.h, d_in, n))
 
     def sync(self):
-        err = C.c_int64(-1)
-        st = self._L.fpx_epaxos_graph_sync(self.h, C.byref(err))
-        if st != 0:
-            raise FpxError(st, err.value)
+        self._host_call(self._L.fpx_epaxos_graph_sync)
 
     def update_executed(self, watermark):
         """updateExecuted of every instance (c, j < watermark[c])"""
         wm = np.ascontiguousarray(watermark, dtype=np.int32)
-        st = self._L.fpx_epaxos_graph_update_executed(self.h, wm.ctypes.data)
-        if st != 0:
-            raise FpxError(st)
+        self._check(self._L.fpx_epaxos_graph_update_executed(self.h, wm.ctypes.data))
 
     def execute_raw(self):
         """(rows [m, 2] of {replica, number}, component heads [m], blockers [n, cap] as 0/1)"""
@@ -453,9 +283,8 @@ class EpaxosGraph:
         out = np.zeros((nv, 2), dtype=np.int32); head = np.zeros(nv, dtype=np.uint8)
         bl = np.zeros((self.n, self.cap), dtype=np.uint8)
         m = C.c_int32(0)
-        st = self._L.fpx_epaxos_graph_execute(self.h, out.ctypes.data, head.ctypes.data, C.byref(m), bl.ctypes.data)
-        if st != 0:
-            raise FpxError(st)
+        self._check(self._L.fpx_epaxos_graph_execute(self.h, out.ctypes.data, head.ctypes.data, C.byref(m),
+                                                     bl.ctypes.data))
         return out[:m.value], head[:m.value], bl
 
     def execute_by_component(self):

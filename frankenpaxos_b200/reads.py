@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .engine import OK, FpxError
+from .engine import _Handle
 
 READS_CLIENT, READS_READ_BATCHER = 0, 1
 READ_OPEN = np.dtype([("key", "<i4"), ("id", "<i4")])
@@ -20,65 +20,37 @@ READ_REQUEST = np.dtype([("slot", "<i4"), ("handle", "<i4")])
 READ_REPLY = np.dtype([("handle", "<i4"), ("reply_slot", "<i4"), ("after_slot", "<i4"), ("reserved", "<i4")])
 
 
-class Reads:
+class Reads(_Handle):
     """One read-quorum tally (kind READS_CLIENT: Client.handleMaxSlotReply, S/multipaxos/Client.scala:851-931;
     READS_READ_BATCHER: ReadBatcher.handleBatchMaxSlotReply, S/multipaxos/ReadBatcher.scala:568-623) and one
     replica's deferred reads (S/multipaxos/Replica.scala:394-529), on `engine`'s GPU."""
 
     def __init__(self, engine, kind=READS_CLIENT, key_capacity=1 << 16, pending_capacity=1 << 16, max_batch=1 << 16):
-        self._L = _lib.lib()
         self.engine, self.kind = engine, kind
         self.key_capacity, self.pending_capacity, self.max_batch = key_capacity, pending_capacity, max_batch
-        self.h = C.c_void_p()
-        st = self._L.fpx_reads_create(C.byref(self.h), engine.h, kind, key_capacity, pending_capacity, max_batch)
-        if st != OK:
-            self.h = None
-            raise FpxError(st)
-
-    def close(self):
-        if getattr(self, "h", None):
-            self._L.fpx_reads_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
-
-    def _check(self, st, idx=-1):
-        if st != OK:
-            raise FpxError(st, idx)
+        super().__init__("fpx_reads_create", "fpx_reads_destroy", engine.h, kind, key_capacity, pending_capacity,
+                         max_batch)
 
     def open(self, keys, ids):
         """A read request per (key, id): MaxSlot(id, {}) / batchMaxSlotReplies(id) = Map()."""
         recs = np.zeros(len(keys), READ_OPEN)
         recs["key"], recs["id"] = keys, ids
-        err = C.c_int64(-1)
-        self._check(self._L.fpx_reads_open(self.h, recs.ctypes.data, len(recs), C.byref(err)), err.value)
+        self._host_call(self._L.fpx_reads_open, recs.ctypes.data, len(recs))
 
     def max_slot_replies(self, recs):
         """Replies in delivery order -> READ_SLOT records of the reads they complete, by completing reply."""
         recs = np.ascontiguousarray(recs, dtype=MAX_SLOT_REPLY)
         out = np.zeros(max(len(recs), 1), READ_SLOT)
-        n, err = C.c_int32(0), C.c_int64(-1)
-        self._check(self._L.fpx_reads_max_slot_replies(self.h, recs.ctypes.data, len(recs), out.ctypes.data, C.byref(n),
-                                                       C.byref(err)), err.value)
+        n = C.c_int32(0)
+        self._host_call(self._L.fpx_reads_max_slot_replies, recs.ctypes.data, len(recs), out.ctypes.data, C.byref(n))
         return out[:n.value].copy()
 
     def replica(self, recs):
         """Read requests in delivery order -> READ_REPLY records of the reads answered now (slot < W)."""
         recs = np.ascontiguousarray(recs, dtype=READ_REQUEST)
         out = np.zeros(max(len(recs), 1), READ_REPLY)
-        n, err = C.c_int32(0), C.c_int64(-1)
-        self._check(self._L.fpx_reads_replica(self.h, recs.ctypes.data, len(recs), out.ctypes.data, C.byref(n),
-                                              C.byref(err)), err.value)
+        n = C.c_int32(0)
+        self._host_call(self._L.fpx_reads_replica, recs.ctypes.data, len(recs), out.ctypes.data, C.byref(n))
         return out[:n.value].copy()
 
     def advance(self, watermark):

@@ -48,7 +48,6 @@ results = {}
 for variant in args.variants.split(","):
     eng = Engine(slot_capacity=S * n, max_batch=3 * n, overflow_capacity=1 << 10, **cfg)
     L = eng._L
-    L.fpx_debug_phase_times.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
     ext = torch.cuda.ExternalStream(eng.stream, device=dev)
     if not args.old_lib:
         eng._check(L.fpx_debug_set_tally_path(eng.h, sum(bit for tok, bit in (("exact", 2), ("nored", 4)) if tok in variant.split("_"))))

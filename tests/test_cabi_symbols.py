@@ -1,34 +1,67 @@
-"""The C-ABI library builds, loads and exports every symbol include/fpx.h declares
-(no compute calls: this runs without a GPU)."""
+"""The C-ABI library builds, loads and exports every symbol include/fpx.h declares, bound with the ctypes types
+of its prototype (no compute calls: this runs without a GPU)."""
 import ctypes
 import os
 import re
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEADER = os.path.join(ROOT, "include", "fpx.h")
+DEBUG_HEADER = os.path.join(ROOT, "frankenpaxos_b200", "csrc", "fpx_debug.h")
 
 
-def declared_symbols():
-    src = open(os.path.join(ROOT, "include", "fpx.h")).read()
+def declared_symbols(path=HEADER):
+    src = open(path).read()
     src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(fpx_[a-z0-9_]+)\s*\(", src)))
+    return sorted(set(re.findall(r"\b(fpx_\w+)\s*\(", src)))
 
 
-def test_header_symbols_exported():
-    from frankenpaxos_b200 import _lib, build
-    path = build.build()
-    L = ctypes.CDLL(path)
-    syms = declared_symbols()
-    assert len(syms) >= 20
-    missing = [s for s in syms if not hasattr(L, s)]
+def mapped(c_type, ret=False):
+    """The ctypes type a C type of the headers is bound with."""
+    if ret and c_type == "const char*":
+        return ctypes.c_char_p
+    if "*" in c_type:
+        return ctypes.c_void_p
+    if ret and c_type == "void":
+        return None
+    return {"int": ctypes.c_int32, "int32_t": ctypes.c_int32, "uint32_t": ctypes.c_uint32,
+            "int64_t": ctypes.c_int64, "float": ctypes.c_float}[c_type]
+
+
+def check_bound(L, path):
+    from frankenpaxos_b200 import _lib
+    protos = _lib.prototypes(path)
+    names = [name for _, name, _ in protos]
+    assert sorted(names) == declared_symbols(path), f"prototypes() skips or invents a declaration of {path}"
+    missing = [s for s in names if not hasattr(L, s)]
     assert not missing, missing
-    assert sorted(_lib.SYMBOLS) == syms, "frankenpaxos_b200/_lib.py binds a different symbol set than fpx.h"
-    assert _lib.lib().fpx_abi_version() == 1
+    for ret, name, params in protos:
+        fn = getattr(L, name)
+        assert fn.argtypes == [mapped(t) for t, _ in params], (name, fn.argtypes)
+        assert fn.restype is mapped(ret, ret=True), (name, fn.restype)
+    return names
+
+
+def test_header_prototypes_exported_and_bound():
+    from frankenpaxos_b200 import _lib
+    L = _lib.lib()
+    assert len(check_bound(L, HEADER)) >= 20
+    assert L.fpx_abi_version() == 1
+
+
+def test_test_aids_exported_and_bound():
+    """The fpx_debug_* aids are declared in fpx_debug.h, not in include/fpx.h, and bound like the ABI."""
+    from frankenpaxos_b200 import _lib
+    names = check_bound(_lib.lib(), DEBUG_HEADER)
+    assert len(names) == 9 and all(n.startswith("fpx_debug_") for n in names)
+    assert not set(names) & set(declared_symbols())
 
 
 def test_struct_layouts_match_header():
     from frankenpaxos_b200 import _lib, engine
     assert ctypes.sizeof(_lib.Config) == 15 * 4
     assert ctypes.sizeof(_lib.SyncResult) == 32
+    assert ctypes.sizeof(_lib.ReadsSyncResult) == 32
+    assert ctypes.sizeof(_lib.EpaxosConfig) == 6 * 4
     assert engine.P2A.itemsize == 16 and engine.P2B.itemsize == 16
     assert engine.CHOSEN.itemsize == 8 and engine.NACK.itemsize == 8
 
