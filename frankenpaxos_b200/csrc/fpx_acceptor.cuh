@@ -31,6 +31,7 @@
 #include <algorithm>
 
 #include "fpx_common.cuh"
+#include "fpx_scan.cuh"
 
 namespace fpx {
 
@@ -152,7 +153,7 @@ __device__ __forceinline__ void acceptor_apply(const AcceptorParams& P, int4* ou
           int leader = __ffs(remaining) - 1;
           int kk = __shfl_sync(full, key, leader);
           bool mine = valid && key == kk;
-          int incl = warp_incl_scan_max(mine ? r : INT_MIN, lane);
+          int incl = warp_incl_scan<ScanMax>(mine ? r : INT_MIN, lane);
           int ex = __shfl_up_sync(full, incl, 1);
           if (lane == 0) ex = INT_MIN;
           if (mine) pin = ex;

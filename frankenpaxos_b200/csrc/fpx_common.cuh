@@ -383,13 +383,4 @@ __device__ __forceinline__ int warp_range_len(int n) {
 }
 __device__ __forceinline__ int4 ld_cg(const int4* p) { return __ldcg(p); }
 
-__device__ __forceinline__ int warp_incl_scan_max(int v, int lane) {
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    int o = __shfl_up_sync(0xffffffffu, v, d);
-    if (lane >= d) v = max(v, o);
-  }
-  return v;
-}
-
 }  // namespace fpx

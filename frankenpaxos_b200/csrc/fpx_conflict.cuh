@@ -16,11 +16,13 @@
 //     sort     the accesses are grouped by row, delivery order kept inside a row (fpx_sort.cuh, stable)
 //     scan     segmented exclusive prefix-max over the sorted accesses, vector state of 2n columns:
 //              block-level segmented scans per 1024-access tile, tile carries chained by one CTA
+//              (tile_carry_kernel, fpx_scan.cuh)
 //     emit     query = resident row (as of before the batch) merged with the exclusive prefix, merged over
 //              the command's keys with atomicMax into deps[i][:]; the last access of a row folds the
 //              row's batch total into the table.
 #pragma once
 #include "fpx_common.cuh"
+#include "fpx_scan.cuh"
 #include "fpx_sort.cuh"
 
 namespace fpx {
@@ -42,7 +44,7 @@ struct CiParams {
   int32_t* acc_cmd;                        // [n_acc]
   uint32_t* perm;                          // [n_acc] accesses sorted by (row, a)
   int32_t* tile_agg;                       // [tiles][2*n_leaders] aggregate of the tile's LAST segment
-  uint32_t* tile_rows;                     // [tiles][2] first / last row of the tile
+  uint32_t* tile_head;                     // [tiles] a row starts in the tile
   int32_t* tile_carry;                     // [tiles][2*n_leaders] prefix entering the tile's FIRST segment
   int32_t* deps_out;                       // [n_cmd][n_leaders]
   DevStatus* st;
@@ -90,105 +92,56 @@ __device__ __forceinline__ int ci_col(const CiParams& P, int cmd) {
   return (P.is_set[cmd] ? 0 : P.n_leaders) + P.leader[cmd];
 }
 
-// Segmented inclusive max-scan of one component over the 1024 sorted accesses of a tile.
-// head = first access of its row inside the tile; s_w is [32][2] scratch.
-__device__ __forceinline__ int ci_tile_scan(int v, bool head, int lane, int warp, int (*s_w)[2]) {
-  int flag = head ? 1 : 0;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    int ov = __shfl_up_sync(0xffffffffu, v, d);
-    int of = __shfl_up_sync(0xffffffffu, flag, d);
-    if (lane >= d) { if (!flag) v = max(v, ov); flag |= of; }
-  }
-  if (lane == 31) { s_w[warp][0] = v; s_w[warp][1] = flag; }
-  __syncthreads();
-  if (warp == 0) {
-    int wv = s_w[lane][0], wf = s_w[lane][1];
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      int ov = __shfl_up_sync(0xffffffffu, wv, d);
-      int of = __shfl_up_sync(0xffffffffu, wf, d);
-      if (lane >= d) { if (!wf) wv = max(wv, ov); wf |= of; }
-    }
-    s_w[lane][0] = wv;   // inclusive over warps 0..lane, restarted at segment heads
-  }
-  __syncthreads();
-  const int pre = warp > 0 ? s_w[warp - 1][0] : 0;
-  __syncthreads();
-  return flag ? v : max(v, pre);   // no head at or before the lane in its warp: the earlier warps' segment goes on
-}
-
-// (2) kPass = 0: aggregate of every tile's last segment + first / last row of the tile.
-//     kPass = 1: exclusive prefixes (+ the carry into the tile's first segment), query merge into
+// (2) kPass = 0: aggregate of every tile's last segment per column, and whether a row starts in the tile.
+//     kPass = 1: exclusive prefixes (with the carry into the tile's first segment), query merge into
 //                deps_out, and the new value of every row (written by the row's last access into tab_new).
 template <int kPass>
 __global__ void __launch_bounds__(kCiTile) ci_scan_kernel(CiParams P) {
-  __shared__ int s_w[32][2];
   __shared__ int s_prev[kCiTile];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int tile = blockIdx.x;
   const int j = tile * kCiTile + tid;                   // position in sorted order
   const bool live = j < P.n_acc;
   const uint32_t a = live ? P.perm[j] : 0u;
   const uint32_t row = live ? P.acc_row[a] : kCiNoRow;
   const int cmd = live ? P.acc_cmd[a] : 0;
-  const uint32_t prev_row = (live && j > 0) ? P.acc_row[P.perm[j - 1]] : kCiNoRow;
-  const bool head = tid == 0 || !live || prev_row != row;   // head within the tile
+  const bool head = live && (j == 0 || P.acc_row[P.perm[j - 1]] != row);   // first access of its row
   const bool real = live && row != kCiNoRow;
   const int my_col = real ? ci_col(P, cmd) : -1;
   const int my_val = real ? P.id[cmd] + 1 : 0;         // TopOne.put: max(id + 1) (:12-15)
   const int nc = 2 * P.n_leaders;
-  const int last = min(kCiTile, P.n_acc - tile * kCiTile) - 1;
   int excl[2 * kCiMaxLeaders];
 #pragma unroll
   for (int c = 0; c < 2 * kCiMaxLeaders; ++c) {
     if (c >= nc) break;
     const int contrib = (my_col == c && P.mode != 2) ? my_val : 0;   // a pure query indexes nothing
-    const int incl = ci_tile_scan(contrib, head, lane, warp, s_w);
-    s_prev[tid] = incl;
+    SegVal<int> x = cta_scan<kCiTile, false>(SegVal<int>{contrib, head}, Seg<ScanMax>());
+    if (kPass == 0) {
+      if (tid == kCiTile - 1) {
+        P.tile_agg[(size_t)tile * nc + c] = x.v;
+        P.tile_head[tile] = x.f;
+      }
+      continue;
+    }
+    const int carry = P.tile_carry[(size_t)tile * nc + c];
+    if (!x.f) x.v = max(x.v, carry);
+    s_prev[tid] = x.v;
     __syncthreads();
-    excl[c] = head ? 0 : s_prev[tid - 1];               // inclusive value of the previous access of the row
+    excl[c] = head ? 0 : (tid == 0 ? carry : s_prev[tid - 1]);   // inclusive value of the previous access of the row
     __syncthreads();
-    if (kPass == 0 && tid == last) P.tile_agg[(size_t)tile * nc + c] = incl;
   }
-  if (kPass == 0) {
-    if (tid == 0) P.tile_rows[tile * 2] = row;
-    if (tid == last) P.tile_rows[tile * 2 + 1] = row;
-    return;
-  }
-  if (!real) return;
-  const uint32_t first_row = P.acc_row[P.perm[tile * kCiTile]];
-  const bool first_seg = row == first_row;              // rows are sorted: the tile's first segment is all of `first_row`
+  if (kPass == 0 || !real) return;
   const bool is_set = P.is_set[cmd] != 0;
   const int32_t* trow = P.tab + (size_t)row * nc;       // as of before the batch: pass 1 never writes `tab`
   const bool last_of_row = (j + 1 >= P.n_acc) || P.acc_row[P.perm[j + 1]] != row;
 #pragma unroll
   for (int c = 0; c < 2 * kCiMaxLeaders; ++c) {
     if (c >= nc) break;
-    int e = excl[c];
-    if (first_seg) e = max(e, P.tile_carry[(size_t)tile * nc + c]);
-    e = max(e, __ldcg(&trow[c]));
+    const int e = max(excl[c], __ldcg(&trow[c]));
     // getTopOneConflicts (:256-300): the sets of the key always, its gets only for a set
     if (P.mode != 1 && (c < P.n_leaders || is_set) && e > 0)
       atomicMax(&P.deps_out[(size_t)cmd * P.n_leaders + (c < P.n_leaders ? c : c - P.n_leaders)], e);
     if (last_of_row && P.mode != 2) P.tab_new[(size_t)row * nc + c] = max(e, my_col == c ? my_val : 0);
-  }
-}
-
-// (2b) carries between tiles: one thread per column walks the tiles in order
-__global__ void ci_carry_kernel(CiParams P, int n_tiles) {
-  const int c = threadIdx.x;
-  const int nc = 2 * P.n_leaders;
-  if (c >= nc) return;
-  int run = 0;
-  uint32_t run_row = kCiNoRow;
-  for (int t = 0; t < n_tiles; ++t) {
-    const uint32_t first = P.tile_rows[t * 2], last = P.tile_rows[t * 2 + 1];
-    const int carry = (first == run_row && first != kCiNoRow) ? run : 0;
-    P.tile_carry[(size_t)t * nc + c] = carry;
-    const int agg = P.tile_agg[(size_t)t * nc + c];
-    run = last == first ? max(carry, agg) : agg;        // one-row tile: the segment goes on; else a new row ended it
-    run_row = last;
   }
 }
 

@@ -20,6 +20,7 @@
 // IntPrefixSet.scala:320-321).  General sets go through depset_union_kernel.
 #pragma once
 #include "fpx_common.cuh"
+#include "fpx_scan.cuh"
 
 namespace fpx {
 
@@ -234,12 +235,17 @@ __global__ void __launch_bounds__(kEpTile) ep_lead_kernel(EpParams P) {
 // read and written as four 128-bit words; largestBallot is reduced per CTA before it touches memory.
 __host__ __device__ __forceinline__ int ep_in_words(const EpGeometry& g, bool accept) { return accept ? 6 + g.n : 6 + 2 * g.n; }
 
+// one atomicMax per CTA of a per-thread ballot key
+__device__ __forceinline__ void ep_cta_max(unsigned long long m, unsigned long long* dst) {
+  m = cta_reduce<kEpTile>(m, ScanMax());
+  if (threadIdx.x == 0 && m) atomicMax(dst, m);
+}
+
 template <bool kAccept>
 __global__ void __launch_bounds__(kEpTile) ep_acceptor_kernel(EpParams P) {
   if (ep_refused(P.s)) return;
   const EpGeometry& g = P.g;
   extern __shared__ int32_t s_ep[];
-  __shared__ unsigned long long s_big[kEpTile / 32];
   const int W = ep_in_words(g, kAccept), Wp = W | 1;
   const int WO = 4 + g.n;                                       // odd: conflict-free as it is
   int32_t* s_in = s_ep;
@@ -330,17 +336,7 @@ __global__ void __launch_bounds__(kEpTile) ep_acceptor_kernel(EpParams P) {
     }
     P.s.proc_ballot[i] = proceeded;
   }
-  // largestBallot of the batch: one atomic per CTA
-  unsigned long long m = proceeded;
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, d));
-  if ((tid & 31) == 0) s_big[tid >> 5] = m;
-  __syncthreads();
-  if (tid == 0) {
-#pragma unroll
-    for (int w = 1; w < kEpTile / 32; ++w) m = max(m, s_big[w]);
-    if (m) atomicMax(P.s.largest + 1, m);
-  }
+  ep_cta_max(proceeded, P.s.largest + 1);   // largestBallot of the batch (its barrier also publishes s_out)
   // replies: coalesced
   int32_t* dst = P.out + tile0 * WO;
   for (int e = tid; e < rows * WO; e += kEpTile) __stcs(dst + e, s_out[e]);
@@ -355,49 +351,22 @@ __global__ void __launch_bounds__(kEpTile) ep_acceptor_kernel(EpParams P) {
 constexpr int kEpScanTile = 1024;
 __global__ void __launch_bounds__(kEpScanTile) ep_nack_tilemax_kernel(EpParams P, unsigned long long* tile_max) {
   if (!(__ldcg(&P.s.st->ts_flags) & 1u)) return;
-  __shared__ unsigned long long s_w[32];
   const int i = blockIdx.x * kEpScanTile + threadIdx.x;
-  unsigned long long m = i < P.n_rec ? P.s.proc_ballot[i] : 0ull;
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, d));
-  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < 32; ++w) m = max(m, s_w[w]);
-    tile_max[blockIdx.x] = m;
-  }
+  const unsigned long long m = cta_reduce<kEpScanTile>(i < P.n_rec ? P.s.proc_ballot[i] : 0ull, ScanMax());
+  if (threadIdx.x == 0) tile_max[blockIdx.x] = m;
 }
 __global__ void __launch_bounds__(kEpScanTile) ep_nack_fixup_kernel(EpParams P, int WO, const unsigned long long* tile_max,
                                                                     int col, bool inclusive, unsigned long long floor) {
   if (!(__ldcg(&P.s.st->ts_flags) & 1u)) return;
-  __shared__ unsigned long long s_w[32];
-  __shared__ unsigned long long s_carry;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   // carry into this tile: largestBallot at batch start and every earlier tile
   unsigned long long c = tid == 0 ? max(P.s.largest[0], floor) : 0ull;
   for (int t = tid; t < (int)blockIdx.x; t += kEpScanTile) c = max(c, tile_max[t]);
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) c = max(c, __shfl_xor_sync(0xffffffffu, c, d));
-  if (lane == 0) s_w[warp] = c;
-  __syncthreads();
-  if (tid == 0) { for (int w = 1; w < 32; ++w) c = max(c, s_w[w]); s_carry = c; }
-  __syncthreads();
+  c = cta_reduce<kEpScanTile>(c, ScanMax());
   const int i = blockIdx.x * kEpScanTile + tid;
   const unsigned long long mine = i < P.n_rec ? P.s.proc_ballot[i] : 0ull;
-  unsigned long long incl = mine;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    unsigned long long o = __shfl_up_sync(0xffffffffu, incl, d);
-    if (lane >= d) incl = max(incl, o);
-  }
-  __syncthreads();
-  if (lane == 31) s_w[warp] = incl;
-  __syncthreads();
-  unsigned long long pre = s_carry;
-  for (int w = 0; w < warp; ++w) pre = max(pre, s_w[w]);
-  unsigned long long excl = __shfl_up_sync(0xffffffffu, incl, 1);
-  if (lane == 0) excl = 0;
-  excl = max(inclusive ? incl : excl, pre);
+  const unsigned long long excl = max(c, inclusive ? cta_scan<kEpScanTile, false>(mine, ScanMax())
+                                                   : cta_scan<kEpScanTile, true>(mine, ScanMax()));
   if (i < P.n_rec) {
     int32_t* o = P.out + (size_t)i * WO;
     if (o[0] == REPLY_NACK) {
@@ -766,19 +735,6 @@ __device__ __forceinline__ void ep_store_rows(int32_t* dst, const int32_t* s_out
   for (int e = threadIdx.x; e < rows * WO; e += kEpTile) {
     const int row = e / WO;
     __stcs(dst + e, s_out[row * WOp + (e - row * WO)]);
-  }
-}
-// one atomicMax per CTA of a per-thread ballot key
-__device__ __forceinline__ void ep_cta_max(unsigned long long m, unsigned long long* dst) {
-  __shared__ unsigned long long s_big[kEpTile / 32];
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, d));
-  if ((threadIdx.x & 31) == 0) s_big[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int w = 1; w < kEpTile / 32; ++w) m = max(m, s_big[w]);
-    if (m) atomicMax(dst, m);
   }
 }
 

@@ -6,7 +6,8 @@
 //   No edge is materialised and no depth-first search is run.  With a(c, j) = w(c, j) for a live (committed,
 //   unexecuted) instance and 0 otherwise, X(v) = the elementwise max of w over v and everything live v reaches
 //   is computed as (DESIGN §6b):
-//     prefix max     P_c[k] = max_{j<k} a(c, j)                       one segmented scan per column
+//     prefix max     P_c[k] = max_{j<k} a(c, j)                       one segmented scan per column: tile maxima,
+//                                                                      tile carries (tile_carry_kernel), tile scans
 //     closure        T0_c[k] = max(k e_c, P_c[k]);  T^{m+1}_c[k] = max_c' T^m_c'[T^m_c[k][c']]   pointer jumping
 //     per vertex     X(v) = max_c T_c[w_c(v)]
 //   v is eligible iff X_c(v) <= A_c (A_c = the column's first absent instance) for every c; with
@@ -19,6 +20,7 @@
 //   k e_c), at and above hi_c nothing is live (T_c[k] = max(k e_c, T_c[hi_c])).
 #pragma once
 #include "fpx_common.cuh"
+#include "fpx_scan.cuh"
 #include "fpx_sort.cuh"
 
 namespace fpx {
@@ -42,7 +44,8 @@ struct EgState {
   int32_t* ids;                        // [n * cap] eligible vertices, (replica, number) order
   int32_t* tile_agg;                   // [tiles * n]
   int32_t* tile_carry;                 // [tiles * n]
-  uint32_t* tile_cnt;                  // [tiles + 1] eligible vertices per tile, then their exclusive scan
+  uint32_t* tile_cnt;                  // [tiles + 1] first the prefix's head flags (1 at a column's first tile), then
+                                       // eligible vertices per tile, then their exclusive scan
   uint32_t* changed;                   // [kEgMaxRounds] round m raised changed[m]; [kEgMaxRounds]: eligible count
   DevStatus* st;
 };
@@ -140,10 +143,8 @@ __global__ void eg_prepare_kernel(EgState S) {
 
 // vector max of the tile, with A_c (first absent) and M_c (largest live watermark, capped at cap) on the side
 __global__ void __launch_bounds__(kEgTile) eg_prefix_tile_kernel(EgState S, EgWin W) {
-  __shared__ int32_t s_w[32][kEgMaxN];
   const int t = blockIdx.x, c = eg_tile_col(W, S.n, t);
   const int j = W.lo[c] + (t - W.tile_off[c]) * kEgTile + threadIdx.x;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   int32_t a[kEgMaxN] = {};
   if (j < W.hi[c]) {
     const size_t v = (size_t)c * S.cap + j;
@@ -159,56 +160,21 @@ __global__ void __launch_bounds__(kEgTile) eg_prefix_tile_kernel(EgState S, EgWi
 #pragma unroll
   for (int q = 0; q < kEgMaxN; ++q) {
     if (q >= S.n) break;
-    int32_t m = a[q];
-    for (int d = 16; d; d >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, d));
-    if (lane == 0) s_w[warp][q] = m;
-  }
-  __syncthreads();
-  if (warp == 0) {
-#pragma unroll
-    for (int q = 0; q < kEgMaxN; ++q) {
-      if (q >= S.n) break;
-      int32_t m = s_w[lane][q];
-      for (int d = 16; d; d >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, d));
-      if (lane == 0) {
-        S.tile_agg[(size_t)t * S.n + q] = m;
-        if (m > 0) atomicMax(&S.win[24 + q], min(m, S.cap));
-      }
+    const int32_t m = cta_reduce<kEgTile>(a[q], ScanMax());
+    if (threadIdx.x == 0) {
+      S.tile_agg[(size_t)t * S.n + q] = m;
+      if (m > 0) atomicMax(&S.win[24 + q], min(m, S.cap));
     }
   }
-}
-
-// exclusive max over the tiles of a column, one warp per column
-__global__ void eg_prefix_carry_kernel(EgState S, EgWin W) {
-  const int c = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (c >= S.n) return;
-  int32_t carry[kEgMaxN] = {};
-  for (int base = W.tile_off[c]; base < W.tile_off[c + 1]; base += 32) {
-    const int t = base + lane;
-    const bool in = t < W.tile_off[c + 1];
-#pragma unroll
-    for (int q = 0; q < kEgMaxN; ++q) {
-      if (q >= S.n) break;
-      int32_t incl = in ? S.tile_agg[(size_t)t * S.n + q] : 0;
-      for (int d = 1; d < 32; d <<= 1) {
-        const int32_t o = __shfl_up_sync(0xffffffffu, incl, d);
-        if (lane >= d) incl = max(incl, o);
-      }
-      int32_t ex = __shfl_up_sync(0xffffffffu, incl, 1);
-      ex = max(carry[q], lane ? ex : 0);
-      if (in) S.tile_carry[(size_t)t * S.n + q] = ex;
-      carry[q] = max(carry[q], __shfl_sync(0xffffffffu, incl, 31));
-    }
-  }
+  if (threadIdx.x == 0) S.tile_cnt[t] = t == W.tile_off[c];   // a column's segment starts with this tile
 }
 
 // T0_c[j + 1] = max((j + 1) e_c, P_c[j + 1]) for every window vertex j; T0_c[lo_c] = lo_c e_c
 __global__ void __launch_bounds__(kEgTile) eg_prefix_apply_kernel(EgState S, EgWin W) {
-  __shared__ int32_t s_w[32][kEgMaxN];
   const int t = blockIdx.x, c = eg_tile_col(W, S.n, t);
   const int j = W.lo[c] + (t - W.tile_off[c]) * kEgTile + threadIdx.x;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const bool in = j < W.hi[c];
+  const bool first = t == W.tile_off[c];   // the column starts here: nothing flows in from earlier tiles
   int32_t a[kEgMaxN] = {};
   if (in) {
     const size_t v = (size_t)c * S.cap + j;
@@ -221,34 +187,15 @@ __global__ void __launch_bounds__(kEgTile) eg_prefix_apply_kernel(EgState S, EgW
 #pragma unroll
   for (int q = 0; q < kEgMaxN; ++q) {
     if (q >= S.n) break;
-    for (int d = 1; d < 32; d <<= 1) {
-      const int32_t o = __shfl_up_sync(0xffffffffu, a[q], d);
-      if (lane >= d) a[q] = max(a[q], o);
-    }
-    if (lane == 31) s_w[warp][q] = a[q];
+    a[q] = cta_scan<kEgTile, false>(a[q], ScanMax());
   }
-  __syncthreads();
-  if (warp == 0) {
-#pragma unroll
-    for (int q = 0; q < kEgMaxN; ++q) {
-      if (q >= S.n) break;
-      int32_t m = s_w[lane][q];
-      for (int d = 1; d < 32; d <<= 1) {
-        const int32_t o = __shfl_up_sync(0xffffffffu, m, d);
-        if (lane >= d) m = max(m, o);
-      }
-      s_w[lane][q] = m;   // inclusive over warps 0..lane
-    }
-  }
-  __syncthreads();
   if (!in) return;
   int32_t* T = S.tab[0];
   const size_t row = (size_t)c * (S.cap + 1);
 #pragma unroll
   for (int q = 0; q < kEgMaxN; ++q) {
     if (q >= S.n) break;
-    int32_t m = max(a[q], S.tile_carry[(size_t)t * S.n + q]);
-    if (warp) m = max(m, s_w[warp - 1][q]);
+    int32_t m = first ? a[q] : max(a[q], S.tile_carry[(size_t)t * S.n + q]);
     if (q == c) m = max(m, j + 1);
     T[(row + j + 1) * S.n + q] = m;
     if (j == W.lo[c]) T[(row + j) * S.n + q] = q == c ? j : 0;
@@ -328,28 +275,13 @@ __global__ void __launch_bounds__(kEgTile) eg_closure_kernel(EgState S, EgWin W,
 }
 
 // eligible vertices to ids[] in (replica, number) order; tile_cnt holds the exclusive scan of the tile counts
-__global__ void __launch_bounds__(kEgTile) eg_compact_kernel(EgState S, EgWin W, int n_tiles) {
-  __shared__ uint32_t s_warp[32];
+__global__ void __launch_bounds__(kEgTile) eg_compact_kernel(EgState S, EgWin W) {
   const int t = blockIdx.x, c = eg_tile_col(W, S.n, t);
   const int j = W.lo[c] + (t - W.tile_off[c]) * kEgTile + threadIdx.x;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const size_t v = (size_t)c * S.cap + j;
   const bool ok = j < W.hi[c] && S.elig[v];
-  const unsigned b = __ballot_sync(0xffffffffu, ok);
-  if (lane == 0) s_warp[warp] = __popc(b);
-  __syncthreads();
-  if (warp == 0) {
-    const uint32_t x = s_warp[lane];
-    uint32_t incl = x;
-    for (int d = 1; d < 32; d <<= 1) {
-      const uint32_t o = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl += o;
-    }
-    s_warp[lane] = incl - x;
-    if (lane == 31 && t == n_tiles - 1) S.changed[kEgMaxRounds] = S.tile_cnt[t] + incl;
-  }
-  __syncthreads();
-  if (ok) S.ids[S.tile_cnt[t] + s_warp[warp] + __popc(b & ((1u << lane) - 1u))] = (int32_t)v;
+  const uint32_t r = cta_scan<kEgTile, true>(ok ? 1u : 0u, ScanSum());
+  if (ok) S.ids[S.tile_cnt[t] + r] = (int32_t)v;
 }
 
 __device__ __forceinline__ bool eg_covered(const EgState& S, int32_t v) {

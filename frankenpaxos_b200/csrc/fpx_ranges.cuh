@@ -16,6 +16,7 @@
 // single-slot kernels use, one (record, chunk) tile per CTA.
 #pragma once
 #include "fpx_common.cuh"
+#include "fpx_scan.cuh"
 
 namespace fpx {
 
@@ -215,10 +216,8 @@ __global__ void __launch_bounds__(kRangeCtaThreads) range_acceptor_kernel(RangeA
                 (rec.w >> 16) * g.per_group + (rec.w & 0xffff) == warp;
         if (match) r = rec.z;
       }
-      int incl = warp_incl_scan_max(r, lane);
-      int prev = __shfl_up_sync(0xffffffffu, incl, 1);
-      if (lane == 0) prev = -1;
-      const int before = max(cur, prev);                       // the acceptor's round when record i is delivered
+      const int incl = warp_incl_scan<ScanMax>(r, lane);
+      const int before = max(cur, warp_excl(incl, lane, -1));  // the acceptor's round when record i is delivered
       if (match) P.dec[i] = r >= before ? kDecAccept : before; // `phase2a.round < round` -> Nack(round) (:245-254)
       cur = max(cur, __shfl_sync(0xffffffffu, incl, 31));      // round = phase2a.round (:259)
     }

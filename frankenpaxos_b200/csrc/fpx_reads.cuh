@@ -7,8 +7,8 @@
 //     keys      sort key = the read key (unknown keys sort last and are skipped)
 //     sort      stable radix sort by key (fpx_sort.cuh): per-key segments in delivery order
 //     scan<0>   tiles of 1024 sorted replies: segmented OR of the replies' voter bits -> tile aggregates
-//     carry     one CTA: exclusive segmented scan of the tile aggregates (a segment may span any
-//               number of tiles)
+//     carry     one CTA (tile_carry_kernel): exclusive segmented scan of the tile aggregates (a
+//               segment may span any number of tiles)
 //     scan<1>   the same OR with the carry: the reply at which the quorum predicate first holds
 //               completes the read (cpos); later replies of the read are ignored
 //     cells     every counted reply (<= cpos) stores {delivery index + 1, slot} with a 64-bit max:
@@ -29,6 +29,7 @@
 //   entry with slot >= W', release the prefix.  All counts live on the device (the _dev forms).
 #pragma once
 #include "fpx_common.cuh"
+#include "fpx_scan.cuh"
 #include "fpx_sort.cuh"
 
 namespace fpx {
@@ -68,7 +69,8 @@ struct ReadTallyParams {
   ReadRow* rows;
   unsigned long long* cells;     // cap x voters
   uint32_t *skey, *perm;
-  uint2* tile_agg;               // {has a segment head, OR since the tile's last head}
+  uint32_t* tile_agg;            // OR since the tile's last head
+  uint32_t* tile_head;           // the tile has a segment head
   uint32_t* carry;               // OR flowing into the tile from earlier tiles
   uint32_t* flag;                // [n] reply i completed its read
   int4* parked;                  // [n] the completion record of reply i
@@ -106,34 +108,6 @@ __global__ void reads_keys_kernel(ReadTallyParams P) {
   P.flag[i] = 0;
 }
 
-// segmented inclusive OR scan over a CTA of kRdTile threads; head = a segment starts here.
-// Returns the inclusive value; *seen = a head at or before this thread within the tile.
-__device__ __forceinline__ uint32_t block_seg_or(uint32_t v, bool head, bool* seen) {
-  __shared__ uint32_t s_v[32], s_f[32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint32_t f = head;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const uint32_t ov = __shfl_up_sync(0xffffffffu, v, d), of = __shfl_up_sync(0xffffffffu, f, d);
-    if (lane >= d) { if (!f) v |= ov; f |= of; }
-  }
-  if (lane == 31) { s_v[warp] = v; s_f[warp] = f; }
-  __syncthreads();
-  if (warp == 0) {
-    uint32_t wv = s_v[lane], wf = s_f[lane];
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const uint32_t ov = __shfl_up_sync(0xffffffffu, wv, d), of = __shfl_up_sync(0xffffffffu, wf, d);
-      if (lane >= d) { if (!wf) wv |= ov; wf |= of; }
-    }
-    s_v[lane] = wv; s_f[lane] = wf;   // inclusive over warps 0..lane
-  }
-  __syncthreads();
-  if (warp > 0 && !f) { v |= s_v[warp - 1]; f = s_f[warp - 1]; }
-  *seen = f != 0;
-  return v;
-}
-
 template <int kPass>
 __global__ void __launch_bounds__(kRdTile) reads_scan_kernel(ReadTallyParams P) {
   __shared__ uint32_t s_incl[kRdTile];
@@ -157,13 +131,13 @@ __global__ void __launch_bounds__(kRdTile) reads_scan_kernel(ReadTallyParams P) 
     if (valid && v >= 0) val = 1u << v;
     if (head) val |= rmask;
   }
-  bool seen;
-  uint32_t incl = block_seg_or(val, head, &seen);
+  const SegVal<uint32_t> x = cta_scan<kRdTile, false>(SegVal<uint32_t>{val, head}, Seg<ScanOr>());
+  uint32_t incl = x.v;
   if (kPass == 0) {
-    if (threadIdx.x == kRdTile - 1) P.tile_agg[blockIdx.x] = make_uint2(seen ? 1u : 0u, incl);
+    if (threadIdx.x == kRdTile - 1) { P.tile_agg[blockIdx.x] = incl; P.tile_head[blockIdx.x] = x.f; }
     return;
   }
-  if (!seen) incl |= P.carry[blockIdx.x];
+  if (!x.f) incl |= P.carry[blockIdx.x];
   s_incl[threadIdx.x] = incl;
   __syncthreads();
   if (!keyed) return;
@@ -179,30 +153,6 @@ __global__ void __launch_bounds__(kRdTile) reads_scan_kernel(ReadTallyParams P) 
   }
   const bool last = j == P.n - 1 || P.skey[P.perm[j + 1]] != k;
   if (last && !reads_quorum(P, incl)) P.rows[k].newmask = incl;
-}
-
-__global__ void __launch_bounds__(1024) reads_carry_kernel(ReadTallyParams P, int tiles) {
-  __shared__ uint32_t s_run;
-  if (threadIdx.x == 0) s_run = 0;
-  __syncthreads();
-  for (int base = 0; base < tiles; base += 1024) {
-    const int t = base + threadIdx.x;
-    const uint2 a = t < tiles ? P.tile_agg[t] : make_uint2(0u, 0u);
-    bool seen;
-    uint32_t incl = block_seg_or(a.y, a.x != 0, &seen);
-    const uint32_t run = s_run;
-    if (!seen) incl |= run;
-    // exclusive = the inclusive value of the previous tile
-    const uint32_t prev = __shfl_up_sync(0xffffffffu, incl, 1);
-    __shared__ uint32_t s_last[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (lane == 31) s_last[warp] = incl;
-    __syncthreads();
-    if (t < tiles) P.carry[t] = lane > 0 ? prev : (warp > 0 ? s_last[warp - 1] : run);
-    __syncthreads();
-    if (threadIdx.x == 1023) s_run = incl;
-    __syncthreads();
-  }
 }
 
 __global__ void reads_cells_kernel(ReadTallyParams P) {
@@ -249,50 +199,19 @@ __global__ void reads_settle_kernel(ReadTallyParams P) {
   row.cpos = -1;
 }
 
-// exclusive scan of one value per thread over a CTA of 1024 threads; *total = the CTA's sum
-__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* total) {
-  __shared__ uint32_t s_w[32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint32_t incl = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const uint32_t o = __shfl_up_sync(0xffffffffu, incl, d);
-    if (lane >= d) incl += o;
-  }
-  __syncthreads();
-  if (lane == 31) s_w[warp] = incl;
-  __syncthreads();
-  if (warp == 0) {
-    const uint32_t w = s_w[lane];
-    uint32_t wi = w;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const uint32_t o = __shfl_up_sync(0xffffffffu, wi, d);
-      if (lane >= d) wi += o;
-    }
-    s_w[lane] = wi;
-  }
-  __syncthreads();
-  *total = s_w[31];
-  return (warp > 0 ? s_w[warp - 1] : 0u) + incl - v;
-}
-
 __global__ void __launch_bounds__(1024) reads_count_kernel(const uint32_t* flag, int n, uint32_t* tile_cnt) {
   const int i = blockIdx.x * 1024 + threadIdx.x;
-  uint32_t total;
-  block_excl_scan(i < n ? flag[i] : 0u, &total);
-  if (threadIdx.x == 0) tile_cnt[blockIdx.x] = total;
+  const int cnt = __syncthreads_count(i < n && flag[i]);   // flags are 0 or 1
+  if (threadIdx.x == 0) tile_cnt[blockIdx.x] = (uint32_t)cnt;
 }
 
-// out[tile_off + rank] = parked[i] for every flagged i; the last tile writes the count to *count
+// out[tile_off + rank] = parked[i] for every flagged i
 __global__ void __launch_bounds__(1024) reads_compact_kernel(const uint32_t* flag, const int4* parked, int n,
-                                                             const uint32_t* tile_off, int4* out, int32_t* count) {
+                                                             const uint32_t* tile_off, int4* out) {
   const int i = blockIdx.x * 1024 + threadIdx.x;
   const uint32_t f = i < n ? flag[i] : 0u;
-  uint32_t total;
-  const uint32_t r = block_excl_scan(f, &total) + tile_off[blockIdx.x];
+  const uint32_t r = cta_scan<1024, true>(f, ScanSum()) + tile_off[blockIdx.x];
   if (f) out[r] = parked[i];
-  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) *count = (int32_t)(tile_off[blockIdx.x] + total);
 }
 
 // ---------------------------------------------------------------------------------- deferred reads
@@ -321,31 +240,27 @@ __global__ void __launch_bounds__(1024) rep_classify_kernel(DeferredParams P) {
     // immediates first in delivery order, then the deferred reads by slot (slot >= W >= 0: slot + 1 fits)
     P.skey[i] = def ? (uint32_t)slot + 1u : 0u;
   }
-  uint32_t total;
-  block_excl_scan(def ? 1u : 0u, &total);
-  if (threadIdx.x == 0) P.tile_cnt[blockIdx.x] = total;
+  const int cnt = __syncthreads_count(def);
+  if (threadIdx.x == 0) P.tile_cnt[blockIdx.x] = (uint32_t)cnt;
 }
 
 // One CTA: total deferred reads, the pool's capacity check (FPX_ERR_OVERFLOW_FULL at the first deferred read
 // that does not fit, nothing of the batch applied), the call's counts.
 __global__ void __launch_bounds__(1024) rep_plan_kernel(DeferredParams P, int tiles) {
-  __shared__ uint32_t s_run, s_hit_tile, s_hit_base;
+  __shared__ uint32_t s_hit_tile, s_hit_base;
   ReadsDev* st = P.st;
   const uint32_t live = st->tail - st->head;
   const uint32_t free_ = (uint32_t)P.pending_cap - live;
-  if (threadIdx.x == 0) { s_run = 0; s_hit_tile = 0xffffffffu; }
-  __syncthreads();
+  uint32_t m = 0;   // deferred reads of the tiles scanned so far
   for (int base = 0; base < tiles; base += 1024) {
     const int t = base + threadIdx.x;
     const uint32_t c = t < tiles ? P.tile_cnt[t] : 0u;
     uint32_t total;
-    const uint32_t off = block_excl_scan(c, &total) + s_run;
+    const uint32_t off = cta_scan<1024, true>(c, ScanSum(), &total) + m;
     if (c > 0 && off <= free_ && free_ < off + c) { s_hit_tile = t; s_hit_base = off; }
-    __syncthreads();
-    if (threadIdx.x == 0) s_run += total;
-    __syncthreads();
+    m += total;
   }
-  const uint32_t m = s_run;
+  __syncthreads();
   if (m <= free_) {
     if (threadIdx.x == 0) {
       st->abort = 0;
@@ -360,8 +275,7 @@ __global__ void __launch_bounds__(1024) rep_plan_kernel(DeferredParams P, int ti
   // the deferred read of rank free_ (delivery order) lies in tile s_hit_tile
   const int i = (int)s_hit_tile * 1024 + threadIdx.x;
   const bool def = i < P.n && P.skey[i] != 0u;
-  uint32_t total;
-  const uint32_t r = block_excl_scan(def ? 1u : 0u, &total) + s_hit_base;
+  const uint32_t r = cta_scan<1024, true>(def ? 1u : 0u, ScanSum()) + s_hit_base;
   if (def && r == free_) reads_error(st, FPX_ERR_OVERFLOW_FULL, i);
   if (threadIdx.x == 0) { st->abort = 1; st->n_replies = 0; }
 }

@@ -5,7 +5,7 @@
 //   sequence of calls, least significant word first.  8 bits per pass, three kernels per pass:
 //     hist     every CTA counts the digits of its contiguous tile of 2048 entries (shared-memory
 //              atomics) -> g_hist[digit][tile]
-//     scan     exclusive scan of g_hist in (digit, tile) order, one CTA
+//     offsets  exclusive scan of g_hist in (digit, tile) order, one CTA (tile_offsets_kernel, fpx_scan.cuh)
 //     scatter  every CTA ranks its tile stably: warp w takes the 32-entry chunks w, w+8, ... of the
 //              tile; inside a chunk __match_any_sync groups equal digits and the rank is the
 //              number of lower lanes in the group; per-(chunk, digit) counts are prefixed over the
@@ -15,6 +15,8 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "fpx_scan.cuh"
 
 namespace fpx {
 
@@ -35,52 +37,6 @@ __global__ void __launch_bounds__(kSortThreads) sort_hist_kernel(const uint32_t*
   }
   __syncthreads();
   g_hist[(size_t)threadIdx.x * n_tiles + tile] = s_h[threadIdx.x];
-}
-
-// exclusive scan of m = 256 * n_tiles counters, one CTA of 1024 threads
-__global__ void __launch_bounds__(1024) sort_scan_kernel(uint32_t* g_hist, int m) {
-  __shared__ uint32_t s_w[32];
-  __shared__ uint32_t s_carry;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) s_carry = 0;
-  __syncthreads();
-  for (int base = 0; base < m; base += 1024 * 4) {
-    uint32_t v[4], sum = 0;
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      int i = base + tid * 4 + u;
-      v[u] = i < m ? g_hist[i] : 0u;
-      sum += v[u];
-    }
-    uint32_t incl = sum;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      uint32_t o = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl += o;
-    }
-    if (lane == 31) s_w[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t w = s_w[lane], wi = w;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        uint32_t o = __shfl_up_sync(0xffffffffu, wi, d);
-        if (lane >= d) wi += o;
-      }
-      s_w[lane] = wi - w;
-    }
-    __syncthreads();
-    uint32_t run = s_carry + s_w[warp] + incl - sum;
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      int i = base + tid * 4 + u;
-      if (i < m) g_hist[i] = run;
-      run += v[u];
-    }
-    __syncthreads();
-    if (tid == 1023) s_carry = run;
-    __syncthreads();
-  }
 }
 
 __global__ void __launch_bounds__(kSortThreads) sort_scatter_kernel(const uint32_t* perm_in, uint32_t* perm_out, const uint32_t* keys,
@@ -140,7 +96,7 @@ static inline int sort_perm_by_key(uint32_t* perm, uint32_t* perm_tmp, const uin
     const int shift = p * 8 < 32 ? p * 8 : 31;   // an extra pass re-sorts by the top bit group: a stable no-op for keys < 2^bits
     const int sh = p * 8 >= 32 ? 31 : shift;
     sort_hist_kernel<<<n_tiles, kSortThreads, 0, stream>>>(src, keys, n, sh, g_hist, n_tiles);
-    sort_scan_kernel<<<1, 1024, 0, stream>>>(g_hist, 256 * n_tiles);
+    tile_offsets_kernel<<<1, 1024, 0, stream>>>(g_hist, 256 * n_tiles, nullptr);
     sort_scatter_kernel<<<n_tiles, kSortThreads, 0, stream>>>(src, dst, keys, n, sh, g_hist, n_tiles);
     uint32_t* t = src; src = dst; dst = t;
   }

@@ -18,6 +18,7 @@
 // `required` field or any malformed byte fails the message (FPX_ERR_WIRE + its index).
 #pragma once
 #include "fpx_common.cuh"
+#include "fpx_scan.cuh"
 
 namespace fpx {
 
@@ -336,61 +337,6 @@ __global__ void __launch_bounds__(kWireEncThreads) wire_size_kernel(WireEncodePa
   }
 }
 
-// pass 2: exclusive scan of the tile sums (one CTA), total at [tiles]
-__global__ void __launch_bounds__(1024) wire_scan_kernel(uint32_t* tile_sum, int tiles, int32_t out_capacity,
-                                                         DevStatus* st) {
-  __shared__ uint32_t s_w[32];
-  __shared__ uint32_t s_carry;
-  if (threadIdx.x == 0) s_carry = 0;
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int base = 0; base < tiles; base += 1024) {
-    int i = base + threadIdx.x;
-    uint32_t v = i < tiles ? tile_sum[i] : 0u, x = v;
-    for (int d = 1; d < 32; d <<= 1) {
-      uint32_t o = __shfl_up_sync(0xffffffffu, x, d);
-      if (lane >= d) x += o;
-    }
-    if (lane == 31) s_w[warp] = x;
-    __syncthreads();
-    uint32_t woff = 0;
-    for (int w = 0; w < warp; ++w) woff += s_w[w];
-    uint32_t excl = s_carry + woff + x - v;
-    __syncthreads();
-    if (i < tiles) tile_sum[i] = excl;
-    if (threadIdx.x == 1023) s_carry = excl + v;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    tile_sum[tiles] = s_carry;
-    if (s_carry > (uint32_t)out_capacity) report_error(st, FPX_ERR_INVALID_ARG, 0);   // output buffer too small
-  }
-}
-
-// CTA-wide exclusive scan of kWireEncPer values per thread (thread-major order = message order
-// i = tile0 + u * threads + t is NOT contiguous per thread, so scan per u-row)
-__device__ __forceinline__ uint32_t cta_excl_scan(uint32_t v, uint32_t* s_w, uint32_t* s_total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint32_t x = v;
-  for (int d = 1; d < 32; d <<= 1) {
-    uint32_t o = __shfl_up_sync(0xffffffffu, x, d);
-    if (lane >= d) x += o;
-  }
-  if (lane == 31) s_w[warp] = x;
-  __syncthreads();
-  const uint32_t wt = lane < kWireEncThreads / 32 ? s_w[lane] : 0u;   // every warp scans the 8 warp totals itself
-  uint32_t wx = wt;
-  for (int d = 1; d < kWireEncThreads / 32; d <<= 1) {
-    uint32_t o = __shfl_up_sync(0xffffffffu, wx, d);
-    if (lane >= d) wx += o;
-  }
-  const uint32_t woff = __shfl_sync(0xffffffffu, wx - wt, warp);
-  const uint32_t tot = __shfl_sync(0xffffffffu, wx, kWireEncThreads / 32 - 1);
-  __syncthreads();
-  *s_total = tot;
-  return woff + x - v;
-}
-
 // pass 2 (Phase2b / Nack).  tile_sum[] holds the byte count of every tile (pass 1); a CTA finds its
 // output offset by summing the counts of the tiles before it straight from L2 (<= a few thousand
 // values: cheaper than a scan kernel or a look-back chain), serialises its tile into shared memory at
@@ -399,10 +345,7 @@ __device__ __forceinline__ uint32_t cta_excl_scan(uint32_t v, uint32_t* s_w, uin
 template <int KIND>
 __global__ void __launch_bounds__(kWireEncThreads) wire_emit_small_kernel(WireEncodeParams P, int tiles) {
   extern __shared__ __align__(16) uint8_t s_out[];   // 16 + tile * max message size
-  __shared__ uint32_t s_w[kWireEncThreads / 32];
-  __shared__ unsigned long long s_pre[kWireEncThreads / 32];
   const int tile = blockIdx.x;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int i0 = tile * kWireEncTile + (int)threadIdx.x * kWireEncPer;
   int4 rec[kWireEncPer];
   uint32_t sz[kWireEncPer];
@@ -429,15 +372,11 @@ __global__ void __launch_bounds__(kWireEncThreads) wire_emit_small_kernel(WireEn
     mine += sz[u];
   }
   // bytes of all tiles before this one (and, for the last tile, the grand total)
-  unsigned long long pre = 0;
-  for (int t = threadIdx.x; t < tile; t += kWireEncThreads) pre += __ldcg(&P.tile_sum[t]);
-  for (int dlt = 16; dlt; dlt >>= 1) pre += __shfl_xor_sync(0xffffffffu, pre, dlt);
-  if (lane == 0) s_pre[warp] = pre;
-  uint32_t run;
-  uint32_t off = cta_excl_scan(mine, s_w, &run);     // (its barriers also publish s_pre)
   unsigned long long gb = 0;
-#pragma unroll
-  for (int w = 0; w < kWireEncThreads / 32; ++w) gb += s_pre[w];
+  for (int t = threadIdx.x; t < tile; t += kWireEncThreads) gb += __ldcg(&P.tile_sum[t]);
+  gb = cta_reduce<kWireEncThreads>(gb, ScanSum());
+  uint32_t run;
+  uint32_t off = cta_scan<kWireEncThreads, true>(mine, ScanSum(), &run);
   const bool fits = gb + run <= (unsigned long long)P.out_capacity;
   if (!fits && gb <= (unsigned long long)P.out_capacity && threadIdx.x == 0)
     report_error(P.st, FPX_ERR_INVALID_ARG, 0);      // output buffer too small
@@ -479,11 +418,13 @@ __global__ void __launch_bounds__(kWireEncThreads) wire_emit_small_kernel(WireEn
 
 // pass 3 (Chosen): header by its thread, value bytes by the warps of the CTA (lane-strided copy)
 __global__ void __launch_bounds__(kWireEncThreads) wire_emit_chosen_kernel(WireEncodeParams P) {
-  __shared__ uint32_t s_w[kWireEncThreads / 32];
   __shared__ uint32_t s_dst[kWireEncTile];     // where each message's value bytes go
   __shared__ int32_t s_src[kWireEncTile], s_len[kWireEncTile];
   const uint32_t tiles = gridDim.x;
-  if (__ldcg(&P.tile_sum[tiles]) > (uint32_t)P.out_capacity) return;
+  if (__ldcg(&P.tile_sum[tiles]) > (uint32_t)P.out_capacity) {   // output buffer too small
+    if (blockIdx.x == 0 && threadIdx.x == 0) report_error(P.st, FPX_ERR_INVALID_ARG, 0);
+    return;
+  }
   const uint32_t gbase = __ldcg(&P.tile_sum[blockIdx.x]);
   uint32_t run = 0;
   for (int u = 0; u < kWireEncPer; ++u) {
@@ -492,7 +433,7 @@ __global__ void __launch_bounds__(kWireEncThreads) wire_emit_chosen_kernel(WireE
     bool bad = false;
     const uint32_t sz = i < P.n ? (uint32_t)wire_size_of<kWireChosen>(P, i, &bad) : 0u;
     uint32_t tot;
-    const uint32_t off = run + cta_excl_scan(sz, s_w, &tot);
+    const uint32_t off = run + cta_scan<kWireEncThreads, true>(sz, ScanSum(), &tot);
     run += tot;
     s_len[slotix] = 0;
     if (i < P.n && !bad) {

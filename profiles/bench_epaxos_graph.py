@@ -7,6 +7,10 @@
            fpx_epaxos_graph (one column, watermark x) and as explicit x -> x - 1 edges in fpx_depgraph; both give
            the same components in the same order.  Host clock around each execute call, and the new handle's
            device time
+  conflict ConflictIndex.batch (QUERY_THEN_PUT) at the size of test_conflict_index_many_tiles_matches_the_oracle:
+           2^17 commands of 8 leaders on one of two hot keys (segments over ~90 and ~40 tiles of the segmented
+           scan).  Host clock around the C call (its copies, kernels and status read-back) from prebuilt arrays,
+           median and best of 20 calls per fresh handle, `--reps` handles
 
 Prints the card name and power limit first, then one JSON line.
     python profiles/bench_epaxos_graph.py [--reps 3]"""
@@ -22,7 +26,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from frankenpaxos_b200 import traces as T  # noqa: E402
-from frankenpaxos_b200.epaxos import DependencyGraph, EpaxosGraph  # noqa: E402
+from frankenpaxos_b200.epaxos import ConflictIndex, DependencyGraph, EpaxosGraph  # noqa: E402
 
 
 def card():
@@ -85,9 +89,32 @@ def chain(reps, L=1 << 18):
             "edges_execute_call_ms": edge_wall * 1e3}
 
 
+def conflict(reps, n=1 << 17, n_leaders=8, calls=20):
+    g = np.random.default_rng(7)
+    pool = g.choice(np.arange(1 << 24), size=2, replace=False).astype(np.int32)
+    keys = g.choice(pool, size=n, p=[0.7, 0.3]).astype(np.int32)   # one key per command
+    off = np.arange(n + 1, dtype=np.int32)
+    lead = g.integers(0, n_leaders, n).astype(np.int32)
+    ids = np.arange(n, dtype=np.int32)
+    sets = (g.random(n) < 0.4).astype(np.uint8)
+    out = np.zeros((n, n_leaders), np.int32)
+    times = []
+    for _ in range(reps):
+        ci = ConflictIndex(n_leaders, key_capacity=1 << 12, max_commands=n, max_keys=n)
+        for c in range(calls + 2):                 # the first two calls warm up
+            t = time.perf_counter()
+            ci._host_call(ci._L.fpx_conflict_index_batch, lead.ctypes.data, ids.ctypes.data, sets.ctypes.data,
+                          off.ctypes.data, keys.ctypes.data, n, ConflictIndex.QUERY_THEN_PUT, out.ctypes.data)
+            if c >= 2:
+                times.append(time.perf_counter() - t)
+        ci.close()
+    return {"commands": n, "leaders": n_leaders, "batch_call_ms_median": float(np.median(times)) * 1e3,
+            "batch_call_ms_best": min(times) * 1e3}
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
     a = ap.parse_args()
     print("card, power limit:", card(), flush=True)
-    print(json.dumps({"cfg4": cfg4(a.reps), "chain": chain(a.reps)}))
+    print(json.dumps({"cfg4": cfg4(a.reps), "chain": chain(a.reps), "conflict": conflict(a.reps)}))

@@ -4,9 +4,9 @@ The multi-block code of these kernels only runs at sizes the other EPaxos tests 
   dependency graph   `dg_execute_kernel` walks its vertices in grid-stride loops (stride = SMs x 1024): at
                      key_capacity = 2^18 every vertex past the first stride is handled in a later iteration
                      than the vertices that depend on it
-  conflict index     carries between 1024-access tiles (`ci_carry_kernel`): hot keys over ~128 tiles, segments
+  conflict index     carries between 1024-access tiles (`tile_carry_kernel`): hot keys over ~128 tiles, segments
                      that end exactly on, one past and one short of a tile boundary, 16 columns (8 leaders), a
-                     near-full table
+                     near-full table, and over 1024 tiles (the carry kernel's chunk of tiles)
   EPaxos handlers    the Nack's largestBallot carried from earlier 1024-record tiles and earlier batches, and the
                      E1 / E2 batch-contract detection across CTAs
   cfg4 round         one PreAccept round at 2^20 instances
@@ -359,26 +359,29 @@ def _ci_shape(g, shape, n, pool):
             counts.append(c); total += c
         keys = np.repeat(g.choice(pool, size=len(counts), replace=False), counts)
         return [[int(k)] for k in g.permutation(keys)] + [[]] * (n - total)
+    if shape == "wide":                                   # 9 of 16 keys per command: over 2^20 accesses, 1152 tiles
+        return [[int(x) for x in g.choice(pool[:16], size=9, replace=False)] for _ in range(n)]
     assert shape == "nearfull"                            # 4000 keys in 4096 rows: probes wrap past row_mask
     return [[int(x) for x in g.choice(pool, size=int(g.integers(0, 4)))] for _ in range(n)]
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("n_leaders", [1, 8])
-@pytest.mark.parametrize("shape", ["hot", "aligned", "aligned+1", "aligned-1", "nearfull"])
+@pytest.mark.parametrize("shape", ["hot", "aligned", "aligned+1", "aligned-1", "nearfull", "wide"])
 def test_conflict_index_many_tiles_matches_the_oracle(shape, n_leaders):
     """2^17 commands per batch: QUERY_THEN_PUT, then PUT, then QUERY, with snapshots in between; every deps row
-    equals KvTopOneConflictIndex.top_one_conflicts bit for bit."""
+    equals KvTopOneConflictIndex.top_one_conflicts bit for bit.  "wide" has more than 1024 tiles of accesses, so
+    its tile carries cross from one 1024-tile chunk of the carry kernel to the next."""
     from frankenpaxos_b200.epaxos import ConflictIndex
     n = 1 << 17
     g = np.random.Generator(np.random.PCG64(1000 + 10 * n_leaders + len(shape)))
-    ci = ConflictIndex(n_leaders, key_capacity=1 << 12, max_commands=n, max_keys=3 * n)
+    ci = ConflictIndex(n_leaders, key_capacity=1 << 12, max_commands=n, max_keys=9 * n)
     ora = O.KvTopOneConflictIndex(n_leaders)
     next_id = [0] * n_leaders
     pool = g.choice(np.arange(-2000, 1 << 24), size=4000, replace=False).astype(np.int32)
     for batch, mode in enumerate((ConflictIndex.QUERY_THEN_PUT, ConflictIndex.PUT, ConflictIndex.QUERY)):
         keys = _ci_shape(g, shape, n, pool)
-        assert sum(map(len, keys)) >= 96 * 1024
+        assert sum(map(len, keys)) >= (1 << 20 if shape == "wide" else 96 * 1024)
         lead = g.integers(0, n_leaders, size=n).astype(np.int32)
         ids = _ci_ids(g, lead, n_leaders, next_id, batch)
         sets = g.random(n) < 0.4
