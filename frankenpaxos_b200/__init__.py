@@ -10,7 +10,8 @@ from .engine import (CHOSEN, NACK, P2A, P2B, Engine, FpxError, dst,  # noqa: F40
                      MULTIPAXOS, MENCIUS, VANILLA_MENCIUS, VM_REPLY_PHASE2B, VM_REPLY_NACK, VM_REPLY_CHOSEN,
                      VM_REPLY_CHOSEN_RETIRED, P2A_RANGE, P2B_RANGE, CHOSEN_RANGE, VM_SKIP, VALUE_NOOP,
                      WIRE_REC, WIRE_PROXYLEADER_INBOUND, WIRE_ACCEPTOR_INBOUND,
-                     WIRE_MENCIUS_PROXYLEADER_INBOUND, WIRE_MENCIUS_ACCEPTOR_INBOUND)
+                     WIRE_MENCIUS_PROXYLEADER_INBOUND, WIRE_MENCIUS_ACCEPTOR_INBOUND, VM_WIRE_CLIENT_REQUEST,
+                     VM_WIRE_PHASE2A, VM_WIRE_PHASE2B, VM_WIRE_SKIP, VM_WIRE_CHOSEN, VM_WIRE_PHASE2_NACK)
 
 from .reads import (Reads, READS_CLIENT, READS_READ_BATCHER, READ_OPEN, MAX_SLOT_REPLY, READ_SLOT,  # noqa: F401
                     READ_REQUEST, READ_REPLY)

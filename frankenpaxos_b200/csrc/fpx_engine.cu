@@ -70,7 +70,7 @@ struct fpx_engine {
   std::vector<cudaEvent_t> step_ev;        // [kStepRing][4], created on first use
   // wire codec staging (grown on demand)
   struct WireBuf { void* p = nullptr; size_t cap = 0; };
-  WireBuf w_bytes, w_offs, w_kind, w_rec, w_out, w_tiles, w_arena, w_voffs;
+  WireBuf w_bytes, w_offs, w_kind, w_rec, w_sender, w_out, w_tiles, w_arena, w_voffs;
   DevStatus* st = nullptr;
   // multi-GPU exchange
   DevExchange* xch = nullptr;          // device copy of the exchange descriptor

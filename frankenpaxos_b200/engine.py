@@ -22,6 +22,8 @@ VALUE_NOOP = -(1 << 31)
 WIRE_REC = np.dtype([("a", "<i4"), ("b", "<i4"), ("c", "<i4"), ("d", "<i4")])
 WIRE_PROXYLEADER_INBOUND, WIRE_ACCEPTOR_INBOUND = 0, 1
 WIRE_MENCIUS_PROXYLEADER_INBOUND, WIRE_MENCIUS_ACCEPTOR_INBOUND = 2, 3
+# ServerInbound members (S/vanillamencius/VanillaMencius.proto:227-241): Engine.wire_decode_vm_server_inbound's kinds
+VM_WIRE_CLIENT_REQUEST, VM_WIRE_PHASE2A, VM_WIRE_PHASE2B, VM_WIRE_SKIP, VM_WIRE_CHOSEN, VM_WIRE_PHASE2_NACK = 1, 4, 5, 6, 7, 9
 
 MULTIPAXOS, MENCIUS, VANILLA_MENCIUS = 0, 1, 2
 # reply kinds of Engine.vm_phase2a (include/fpx.h FPX_VM_REPLY_*)
@@ -371,6 +373,71 @@ class Engine(_Handle):
         cap = int(24 * len(recs) + lens[recs["value_id"][ok]].sum()) + 16
         return self._wire_encode(self._L.fpx_wire_encode_chosen, recs, CHOSEN, 0, arena.ctypes.data if len(arena) else None,
                                  value_offsets.ctypes.data, len(value_offsets) - 1, cap)
+
+    # -- vanilla Mencius wire codec (protocol=VANILLA_MENCIUS): ServerInbound bytes <-> records (include/fpx.h)
+    def wire_decode_vm_server_inbound(self, buf, offsets):
+        """Returns (kind[n], rec[n], sender[n]): kind = the ServerInbound member's field number, sender = the
+        server field of a Phase2a / Phase2b / Skip, else -1."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offsets = np.ascontiguousarray(offsets, dtype=np.int32)
+        n = len(offsets) - 1
+        kind = np.zeros(max(n, 1), dtype=np.int32)
+        rec = np.zeros(max(n, 1), dtype=WIRE_REC)
+        sender = np.zeros(max(n, 1), dtype=np.int32)
+        self._host_call(self._L.fpx_wire_decode_vm_server_inbound, buf.ctypes.data if len(buf) else None,
+                        offsets.ctypes.data, n, kind.ctypes.data, rec.ctypes.data, sender.ctypes.data)
+        return kind[:n], rec[:n], sender[:n]
+
+    def _wire_encode_valued(self, fn, recs, dtype, value_ids, arena, value_offsets):
+        """An encoder whose messages carry a CommandOrNoop: value_id v is arena[value_offsets[v] ..
+        value_offsets[v+1]), VALUE_NOOP the Noop."""
+        arena = np.zeros(0, dtype=np.uint8) if arena is None else np.ascontiguousarray(arena, dtype=np.uint8)
+        value_offsets = np.zeros(1, dtype=np.int32) if value_offsets is None else \
+            np.ascontiguousarray(value_offsets, dtype=np.int32)
+        lens = np.diff(value_offsets)
+        ok = (value_ids >= 0) & (value_ids < len(lens))
+        cap = int(48 * len(recs) + lens[value_ids[ok]].sum()) + 16   # 48: the longest head (Phase2a)
+        return self._wire_encode(fn, recs, dtype, 0, arena.ctypes.data if len(arena) else None,
+                                 value_offsets.ctypes.data, len(value_offsets) - 1, cap)
+
+    def wire_encode_vm_replies(self, replies, arena=None, value_offsets=None):
+        """The dense reply stream of vm_phase2a / vm_step_dev -> (bytes, offsets[n+1]); a kind-3 reply
+        (VM_REPLY_CHOSEN_RETIRED) is a zero-length message: the caller holds that slot's value."""
+        replies = np.ascontiguousarray(replies, dtype=P2B)
+        vids = np.where(replies["group"] == VM_REPLY_CHOSEN, replies["round"], -1)
+        return self._wire_encode_valued(self._L.fpx_wire_encode_vm_replies, replies, P2B, vids, arena, value_offsets)
+
+    def wire_encode_vm_chosen(self, recs, arena=None, value_offsets=None):
+        recs = np.ascontiguousarray(recs, dtype=CHOSEN)
+        return self._wire_encode_valued(self._L.fpx_wire_encode_vm_chosen, recs, CHOSEN, recs["value_id"], arena,
+                                        value_offsets)
+
+    def wire_encode_vm_phase2a(self, recs, arena=None, value_offsets=None):
+        """Client-request records -> the coordinator's Phase2a (sending_server = slot mod n)."""
+        recs = np.ascontiguousarray(recs, dtype=P2A)
+        return self._wire_encode_valued(self._L.fpx_wire_encode_vm_phase2a, recs, P2A, recs["value_id"], arena,
+                                        value_offsets)
+
+    def wire_encode_vm_skip(self, recs):
+        return self._wire_encode(self._L.fpx_wire_encode_vm_skip, recs, VM_SKIP, 46)
+
+    def wire_decode_vm_server_inbound_dev(self, d_bytes, d_offsets, n, d_kind, d_out, d_sender):
+        self._check(self._L.fpx_wire_decode_vm_server_inbound_dev(self.h, d_bytes, d_offsets, n, d_kind, d_out, d_sender))
+
+    def wire_encode_vm_replies_dev(self, d_in, n, d_arena, d_value_offsets, num_values, d_out, out_capacity, d_offsets):
+        self._check(self._L.fpx_wire_encode_vm_replies_dev(self.h, d_in, n, d_arena, d_value_offsets, num_values, d_out,
+                                                           out_capacity, d_offsets))
+
+    def wire_encode_vm_chosen_dev(self, d_in, n, d_arena, d_value_offsets, num_values, d_out, out_capacity, d_offsets):
+        self._check(self._L.fpx_wire_encode_vm_chosen_dev(self.h, d_in, n, d_arena, d_value_offsets, num_values, d_out,
+                                                          out_capacity, d_offsets))
+
+    def wire_encode_vm_phase2a_dev(self, d_in, n, d_arena, d_value_offsets, num_values, d_out, out_capacity, d_offsets):
+        self._check(self._L.fpx_wire_encode_vm_phase2a_dev(self.h, d_in, n, d_arena, d_value_offsets, num_values, d_out,
+                                                           out_capacity, d_offsets))
+
+    def wire_encode_vm_skip_dev(self, d_in, n, d_out, out_capacity, d_offsets):
+        self._check(self._L.fpx_wire_encode_vm_skip_dev(self.h, d_in, n, d_out, out_capacity, d_offsets))
 
     def vm_client_request_dev(self, d_in, n):
         self._check(self._L.fpx_vm_client_request_dev(self.h, d_in, n))

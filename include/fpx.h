@@ -426,6 +426,68 @@ int fpx_wire_encode_chosen(fpx_engine* e, const fpx_chosen* in, int32_t n, const
                            const int32_t* value_offsets, int32_t num_values, uint8_t* out, int32_t out_capacity,
                            int32_t* offsets, int64_t* err_index);
 
+/* ---- Wire codec of vanilla Mencius (protocol FPX_VANILLA_MENCIUS; any other: FPX_ERR_UNSUPPORTED) ----
+ * S/vanillamencius/VanillaMencius.proto: ServerInbound :227-241 {client_request = 1, phase1a = 2, phase1b = 3,
+ * phase2a = 4, phase2b = 5, skip = 6, chosen = 7, phase1_nack = 8, phase2_nack = 9}, CommandOrNoop :84-93
+ * {command = 1, noop = 2}, ClientRequest :95-100, Phase2a :154-162, Skip :164-172, Phase2b :174-181, Chosen
+ * :183-190 (isRevocation is a required bool), Phase2Nack :209-215.  Parsing rules, buffers, offsets[n+1] and
+ * out_capacity as for the calls above; n (servers) = acceptors_per_group.
+ *
+ * Decode: kind[i] = the oneof member's field number (0: none); sender[i] = the message's server field
+ * (Phase2a.sending_server, which handlePhase2a :1055 compares with the slot's owner; Phase2b / Skip
+ * server_index), -1 for the other members.  out[i] per kind:
+ *   1 client_request  {0, 0, value_off, value_len}: the whole `command` field, tag and length included.
+ *                     Those bytes are CommandOrNoop().withCommand(command) (both carry Command as field 1):
+ *                     the arena entry of the Phase2a the coordinator sends.
+ *   4 phase2a         {slot, round, value_off, value_len}: the CommandOrNoop, never read
+ *   5 phase2b         {0, server_index, slot, round}: the fpx_p2b fpx_proxyleader_phase2b takes
+ *   6 skip            {server_index, start, stop, 0}: an fpx_vm_skip_rec once the caller sets server and own
+ *   7 chosen          {slot, is_revocation (0 / 1), value_off, value_len}
+ *   9 phase2_nack     {slot, round, 0, 0}
+ *   2, 3, 8 and unknown members: {0, 0, body_off, body_len} for the host.
+ * A missing required field (isRevocation and command_or_noop included), a second command_or_noop or
+ * `command`, or a group wire type is FPX_ERR_WIRE at the message's index. */
+int fpx_wire_decode_vm_server_inbound(fpx_engine* e, const uint8_t* bytes, const int32_t* offsets, int32_t n,
+                                      int32_t* kind, fpx_wire_rec* out, int32_t* sender, int64_t* err_index);
+int fpx_wire_decode_vm_server_inbound_dev(fpx_engine* e, const uint8_t* d_bytes, const int32_t* d_offsets, int32_t n,
+                                          int32_t* d_kind, fpx_wire_rec* d_out, int32_t* d_sender);
+/* Encoders: canonical ServerInbound bytes, one message per record.  Values: value_id v is the CommandOrNoop
+ * arena[value_offsets[v] .. value_offsets[v+1]); FPX_VALUE_NOOP is CommandOrNoop{noop {}} (bytes 12 00); any
+ * other value_id outside [0, num_values) is FPX_ERR_INVALID_ARG at that record.  isRevocation is always written
+ * false (18 00): the engine has no revocation.
+ * _vm_replies: the dense reply stream of fpx_vm_phase2a[_dev] / fpx_vm_step_dev, by reply kind:
+ *   0 phase2b{server_index = acceptor, slot, round}   1 phase2_nack{slot, round}
+ *   2 chosen{slot, command_or_noop = the value in `round`, false}
+ *   3 (FPX_VM_REPLY_CHOSEN_RETIRED) a ZERO-LENGTH message: the engine no longer holds the retired slot's value;
+ *     the caller, which holds the executed entry, sends that Chosen itself.
+ *   Any other kind is FPX_ERR_INVALID_ARG at that record. */
+int fpx_wire_encode_vm_replies(fpx_engine* e, const fpx_p2b* in, int32_t n, const uint8_t* arena,
+                               const int32_t* value_offsets, int32_t num_values, uint8_t* out, int32_t out_capacity,
+                               int32_t* offsets, int64_t* err_index);
+int fpx_wire_encode_vm_replies_dev(fpx_engine* e, const fpx_p2b* d_in, int32_t n, const uint8_t* d_arena,
+                                   const int32_t* d_value_offsets, int32_t num_values, uint8_t* d_out,
+                                   int32_t out_capacity, int32_t* d_offsets);
+/* chosen{slot, value, false} per tally output (handlePhase2b :1127-1135 sends it to every other server). */
+int fpx_wire_encode_vm_chosen(fpx_engine* e, const fpx_chosen* in, int32_t n, const uint8_t* arena,
+                              const int32_t* value_offsets, int32_t num_values, uint8_t* out, int32_t out_capacity,
+                              int32_t* offsets, int64_t* err_index);
+int fpx_wire_encode_vm_chosen_dev(fpx_engine* e, const fpx_chosen* d_in, int32_t n, const uint8_t* d_arena,
+                                  const int32_t* d_value_offsets, int32_t num_values, uint8_t* d_out,
+                                  int32_t out_capacity, int32_t* d_offsets);
+/* phase2a{sending_server = slot mod n (in [0, n)), slot, round, value} per client-request record
+ * (handleClientRequest :806-815); dst is not on the wire. */
+int fpx_wire_encode_vm_phase2a(fpx_engine* e, const fpx_p2a* in, int32_t n, const uint8_t* arena,
+                               const int32_t* value_offsets, int32_t num_values, uint8_t* out, int32_t out_capacity,
+                               int32_t* offsets, int64_t* err_index);
+int fpx_wire_encode_vm_phase2a_dev(fpx_engine* e, const fpx_p2a* d_in, int32_t n, const uint8_t* d_arena,
+                                   const int32_t* d_value_offsets, int32_t num_values, uint8_t* d_out,
+                                   int32_t out_capacity, int32_t* d_offsets);
+/* skip{server_index = server, start, stop}; own is not on the wire. */
+int fpx_wire_encode_vm_skip(fpx_engine* e, const fpx_vm_skip_rec* in, int32_t n, uint8_t* out, int32_t out_capacity,
+                            int32_t* offsets, int64_t* err_index);
+int fpx_wire_encode_vm_skip_dev(fpx_engine* e, const fpx_vm_skip_rec* d_in, int32_t n, uint8_t* d_out,
+                                int32_t out_capacity, int32_t* d_offsets);
+
 /* ---- EPaxos replica (S/epaxos/Replica.scala) ------------------------------
  * One fpx_epaxos handle = one replica's cmdLog (:298-330) and leaderStates
  * (:347-386) for n = 2f+1 replicas, instances (replicaIndex, instanceNumber <
