@@ -1279,5 +1279,6 @@ int fpx_snapshot_log(fpx_engine* e, int32_t first_slot, int32_t n_slots, int32_t
 }  // extern "C"
 
 #include "fpx_engine_epaxos.inc"
+#include "fpx_engine_epaxos_wire.inc"
 #include "fpx_engine_f4.inc"
 #include "fpx_engine_reads.inc"

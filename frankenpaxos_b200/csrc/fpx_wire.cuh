@@ -22,6 +22,7 @@
 // `required` field or any malformed byte fails the message (FPX_ERR_WIRE + its index).
 #pragma once
 #include "fpx_common.cuh"
+#include "fpx_epaxos.cuh"
 #include "fpx_scan.cuh"
 
 namespace fpx {
@@ -233,6 +234,34 @@ struct WireDecodeParams {
   DevStatus* st;
 };
 
+// The byte span of a decoder CTA's messages [m0, m1): staged in s_buf (kWireStage + 32 bytes) when it fits,
+// window byte 0 = buffer byte `base`.  Every thread of the CTA calls it (it ends with __syncthreads).
+struct WireSpan {
+  long long lo, hi, base;
+  bool sane, staged;
+};
+__device__ __forceinline__ WireSpan wire_stage_span(const uint8_t* bytes, const int32_t* offs, int n, int m0, int m1,
+                                                    uint8_t* s_buf) {
+  WireSpan w;
+  w.lo = offs[m0]; w.hi = offs[m1];
+  const long long total = offs[n];
+  w.base = w.lo & ~15ll;
+  w.sane = w.lo >= 0 && w.lo <= w.hi && w.hi <= total;   // garbage offsets never turn into wild reads
+  w.staged = w.sane && w.hi - w.base <= kWireStage;
+  if (w.staged) {
+    // 128-bit loads while the chunk lies inside the buffer, bytes for the last partial chunk
+    for (long long k = (long long)threadIdx.x * 16; w.base + k < w.hi; k += (long long)kWireDecThreads * 16) {
+      if (w.base + k + 16 <= (total & ~15ll)) {
+        *(uint4*)(s_buf + k) = __ldg((const uint4*)(bytes + w.base + k));
+      } else {
+        for (int j = 0; j < 16 && w.base + k + j < total; ++j) s_buf[k + j] = __ldg(bytes + w.base + k + j);
+      }
+    }
+  }
+  __syncthreads();
+  return w;
+}
+
 // kVm: the vanilla Mencius instantiation (inbound 4); the other inbounds' instantiation compiles without its bool,
 // sender and ClientRequest span
 template <bool kVm>
@@ -241,22 +270,9 @@ __global__ void __launch_bounds__(kWireDecThreads) wire_decode_kernel(WireDecode
   __shared__ __align__(16) uint8_t s_buf[kWireStage + 32];
   const int m0 = blockIdx.x * kWireDecThreads;
   const int m1 = min(P.n, m0 + kWireDecThreads);
-  const long long lo = P.offs[m0], hi = P.offs[m1];
-  const long long total = P.offs[P.n];
-  const long long base = lo & ~15ll;
-  const bool sane = lo >= 0 && lo <= hi && hi <= total;   // garbage offsets never turn into wild reads
-  const bool staged = sane && hi - base <= kWireStage;
-  if (staged) {
-    // 128-bit loads while the chunk lies inside the buffer, bytes for the last partial chunk
-    for (long long k = (long long)threadIdx.x * 16; base + k < hi; k += (long long)kWireDecThreads * 16) {
-      if (base + k + 16 <= (total & ~15ll)) {
-        *(uint4*)(s_buf + k) = __ldg((const uint4*)(P.bytes + base + k));
-      } else {
-        for (int j = 0; j < 16 && base + k + j < total; ++j) s_buf[k + j] = __ldg(P.bytes + base + k + j);
-      }
-    }
-  }
-  __syncthreads();
+  const WireSpan w = wire_stage_span(P.bytes, P.offs, P.n, m0, m1, s_buf);
+  const long long lo = w.lo, hi = w.hi, base = w.base;
+  const bool sane = w.sane, staged = w.staged;
   const int i = m0 + threadIdx.x;
   if (i >= m1) return;
   const long long a = P.offs[i], b = P.offs[i + 1];
@@ -278,6 +294,398 @@ __global__ void __launch_bounds__(kWireDecThreads) wire_decode_kernel(WireDecode
   P.kind[i] = kind;
   P.out[i] = rec;
   if (kVm) P.sender[i] = ok ? sender : -1;
+}
+
+// ---------------------------------------------------------------------------
+// EPaxos ReplicaInbound (S/epaxos/EPaxos.proto:220-235): one thread per message as above, with a nested parser.
+// The members' fields are nested messages (Instance :35-41, Ballot :46-52, CommandOrNoop :80-88 over Command
+// :61-78, InstancePrefixSetProto :97-103 over IntPrefixSetProto) or int32s.  Parsed as protobuf-java's
+// mergeFrom builds the message: a member given again merges into the one before it (a nested Instance / Ballot
+// too: the have-bits accumulate, a later scalar wins), another member starts afresh, and `required` is checked on
+// the message that results.  Every member body on the wire is parsed, so malformed bytes anywhere fail.
+// ---------------------------------------------------------------------------
+// decoded row (12 + n int32, include/fpx.h fpx_epaxos_wire_decode)
+enum { EW_IREP = 0, EW_INUM, EW_BORD, EW_BREP, EW_REPLICA, EW_VBORD, EW_VBREP, EW_STATUS, EW_VALUE, EW_SEQ, EW_FLAGS,
+       EW_OVERFLOW, EW_DEPS };
+// what a member's field is: nested messages first (wire type 2), then the int32 fields (wire type 0)
+enum { kEfNone = 0, kEfInstance, kEfBallot, kEfVote, kEfValue, kEfDeps, kEfReplica, kEfStatus, kEfSeq };
+// the roles of fields 1..8 of member `which`, a nibble each (field 1 lowest)
+__device__ __forceinline__ uint32_t ep_wire_roles(int which) {
+  switch (which) {
+    case 1: return 0x4u;              // ClientRequest{command}: the value
+    case 2:                           // PreAccept / Accept {instance, ballot, command_or_noop, sequence_number,
+    case 4: return 0x58421u;          //   dependencies}
+    case 3: return 0x58621u;          // PreAcceptOk {instance, ballot, replica_index, sequence_number, dependencies}
+    case 5: return 0x6000210u;        // AcceptOk {instance = 2, ballot = 3, replica_index = 7}
+    case 6: return 0x5841u;           // Commit {instance, command_or_noop, sequence_number, dependencies}
+    case 7:                           // Prepare / Nack {instance, ballot (largest_ballot)}
+    case 9: return 0x21u;
+    case 8: return 0x58473612u;       // PrepareOk {ballot, instance, replica_index, vote_ballot, status,
+                                      //   [command_or_noop, sequence_number, dependencies]}
+    default: return 0u;
+  }
+}
+// have-bits of the nested messages (EpWireMsg::sub)
+enum { kSubInstance = 0x3, kSubBallot = 0xc, kSubVote = 0x30, kSubNumReplicas = 0x40 };
+
+struct EpWireMsg {
+  int irep, inum, bord, brep, vord, vrep, replica, status, seq;
+  unsigned have;          // fields of the member given (bit f - 1)
+  unsigned sub;           // kSub*
+  int num_replicas, dcount, overflow;
+  uint32_t voff, vlen;    // the value's span (reader positions)
+  bool noop;
+};
+__device__ __forceinline__ EpWireMsg ep_wire_fresh() {
+  EpWireMsg m;
+  m.irep = m.inum = m.bord = m.brep = m.vord = m.vrep = -1;
+  m.replica = m.status = m.seq = 0;
+  m.have = m.sub = 0;
+  m.num_replicas = m.dcount = m.overflow = 0;
+  m.voff = m.vlen = 0;
+  m.noop = false;
+  return m;
+}
+
+// A message whose known fields are all skipped: bit f - 1 of *have for field f <= 4 given with its wire type
+// (wt2: the length-delimited ones, wt0: the varints).  Command (wt2 0x9, wt0 0x6) and Noop (none).
+template <bool kS>
+__device__ __forceinline__ bool ep_wire_fields(WireReader<kS> b, unsigned wt2, unsigned wt0, unsigned* have) {
+  while (!b.done()) {
+    const uint32_t tag = b.tag();
+    if (!b.ok) return false;
+    const int f = (int)(tag >> 3), wt = (int)(tag & 7);
+    if (f <= 4 && (((wt == 2 ? wt2 : wt == 0 ? wt0 : 0u) >> (f - 1)) & 1u)) *have |= 1u << (f - 1);
+    if (!b.skip(wt)) return false;
+  }
+  return true;
+}
+// Instance / Ballot: two int32 fields, merged into (*x, *y) and have-bits << shift
+template <bool kS>
+__device__ __forceinline__ bool ep_wire_pair(WireReader<kS> b, int* x, int* y, unsigned* have, int shift) {
+  while (!b.done()) {
+    const uint32_t tag = b.tag();
+    if (!b.ok) return false;
+    const int f = (int)(tag >> 3), wt = (int)(tag & 7);
+    if (wt == 0 && (f == 1 || f == 2)) {
+      const int v = (int)b.int32();
+      if (!b.ok) return false;
+      if (f == 1) *x = v; else *y = v;
+      *have |= 1u << (shift + f - 1);
+    } else if (!b.skip(wt)) {
+      return false;
+    }
+  }
+  return true;
+}
+// CommandOrNoop {command = 1, noop = 2}: the last member wins, a Command given again merges
+template <bool kS>
+__device__ __forceinline__ bool ep_wire_value(WireReader<kS> b, bool* noop) {
+  int which = 0;
+  unsigned cmd = 0;
+  while (!b.done()) {
+    const uint32_t tag = b.tag();
+    if (!b.ok) return false;
+    const int f = (int)(tag >> 3), wt = (int)(tag & 7);
+    if (wt == 2 && (f == 1 || f == 2)) {
+      const uint32_t n = b.small();
+      if (!b.ok || b.end - b.p < n) return false;
+      WireReader<kS> s = b;
+      s.end = b.p + n;
+      if (f == 1 && which != 1) cmd = 0;
+      unsigned none = 0;
+      if (!(f == 1 ? ep_wire_fields(s, 0x9u, 0x6u, &cmd) : ep_wire_fields(s, 0u, 0u, &none))) return false;
+      which = f;
+      b.p += n;
+    } else if (!b.skip(wt)) {
+      return false;
+    }
+  }
+  *noop = which == 2;
+  return which != 1 || cmd == 0xfu;        // Command's four fields are required
+}
+// IntPrefixSetProto {watermark = 1, repeated value = 2}: `value` packed or not; *values counts them
+template <bool kS>
+__device__ __forceinline__ bool ep_wire_prefix_set(WireReader<kS> b, int* watermark, int* values) {
+  bool have = false;
+  while (!b.done()) {
+    const uint32_t tag = b.tag();
+    if (!b.ok) return false;
+    const int f = (int)(tag >> 3), wt = (int)(tag & 7);
+    if (f == 1 && wt == 0) {
+      *watermark = (int)b.int32();
+      have = true;
+    } else if (f == 2 && wt == 0) {
+      b.int32();
+      ++*values;
+    } else if (f == 2 && wt == 2) {
+      const uint32_t n = b.small();
+      if (!b.ok || b.end - b.p < n) return false;
+      WireReader<kS> s = b;
+      s.end = b.p + n;
+      while (!s.done()) {
+        s.int32();
+        if (!s.ok) return false;
+        ++*values;
+      }
+      b.p = s.p;
+    } else {
+      b.skip(wt);
+    }
+    if (!b.ok) return false;
+  }
+  return have;
+}
+// InstancePrefixSetProto {numReplicas = 1, repeated int_prefix_set = 2}: entry k's watermark -> deps[k] (k < n)
+template <bool kS>
+__device__ __forceinline__ bool ep_wire_deps(WireReader<kS> b, EpWireMsg& m, int32_t* deps, int n) {
+  while (!b.done()) {
+    const uint32_t tag = b.tag();
+    if (!b.ok) return false;
+    const int f = (int)(tag >> 3), wt = (int)(tag & 7);
+    if (f == 1 && wt == 0) {
+      m.num_replicas = (int)b.int32();
+      if (!b.ok) return false;
+      m.sub |= kSubNumReplicas;
+    } else if (f == 2 && wt == 2) {
+      const uint32_t len = b.small();
+      if (!b.ok || b.end - b.p < len) return false;
+      WireReader<kS> s = b;
+      s.end = b.p + len;
+      int wm = 0;
+      if (!ep_wire_prefix_set(s, &wm, &m.overflow)) return false;
+      if (m.dcount < n) deps[m.dcount] = wm;
+      ++m.dcount;
+      b.p += len;
+    } else if (!b.skip(wt)) {
+      return false;
+    }
+  }
+  return true;
+}
+// one body of member `which`, merged into m
+template <bool kS>
+__device__ __forceinline__ bool ep_wire_member(WireReader<kS> b, int which, int n, EpWireMsg& m, int32_t* deps) {
+  const uint32_t roles = ep_wire_roles(which);
+  while (!b.done()) {
+    const uint32_t tpos = b.p;
+    const uint32_t tag = b.tag();
+    if (!b.ok) return false;
+    const int f = (int)(tag >> 3), wt = (int)(tag & 7);
+    const int role = f <= 8 ? (int)((roles >> (4 * (f - 1))) & 15u) : kEfNone;
+    if (role == kEfNone || wt != (role >= kEfReplica ? 0 : 2)) {    // unknown, or a known number with another type
+      if (!b.skip(wt)) return false;
+      continue;
+    }
+    const unsigned bit = 1u << (f - 1);
+    if (role >= kEfReplica) {
+      const int v = (int)b.int32();
+      if (!b.ok) return false;
+      if (role == kEfReplica) m.replica = v; else if (role == kEfStatus) m.status = v; else m.seq = v;
+      m.have |= bit;
+      continue;
+    }
+    const uint32_t len = b.small();
+    if (!b.ok || b.end - b.p < len) return false;
+    WireReader<kS> s = b;
+    s.end = b.p + len;
+    bool ok;
+    if (role == kEfInstance) {
+      ok = ep_wire_pair(s, &m.irep, &m.inum, &m.sub, 0);
+    } else if (role == kEfBallot) {
+      ok = ep_wire_pair(s, &m.bord, &m.brep, &m.sub, 2);
+    } else if (role == kEfVote) {
+      ok = ep_wire_pair(s, &m.vord, &m.vrep, &m.sub, 4);
+    } else if (role == kEfDeps) {
+      ok = ep_wire_deps(s, m, deps, n);
+    } else if (m.have & bit) {
+      ok = false;                     // a second command_or_noop (or ClientRequest.command) would merge: unsupported
+    } else if (which == 1) {          // ClientRequest: the whole `command` field = CommandOrNoop().withCommand(command)
+      unsigned cmd = 0;
+      ok = ep_wire_fields(s, 0x9u, 0x6u, &cmd) && cmd == 0xfu;
+      m.voff = tpos; m.vlen = s.end - tpos; m.noop = false;
+    } else {
+      ok = ep_wire_value(s, &m.noop);
+      m.voff = s.p; m.vlen = len;
+    }
+    if (!ok) return false;
+    m.have |= bit;
+    b.p += len;
+  }
+  return true;
+}
+// One ReplicaInbound -> FPX_OK / FPX_ERR_WIRE / FPX_ERR_UNSUPPORTED (a set of another size, an unknown status)
+template <bool kS>
+__device__ __forceinline__ int ep_wire_decode_one(WireReader<kS> r, int n, int* kind, EpWireMsg& m, int32_t* deps) {
+  int which = 0;
+  while (!r.done()) {
+    const uint32_t tag = r.tag();
+    if (!r.ok) return FPX_ERR_WIRE;
+    const int wt = (int)(tag & 7);
+    if (wt == 2) {
+      const uint32_t len = r.small();
+      if (!r.ok || r.end - r.p < len) return FPX_ERR_WIRE;
+      const int f = (int)(tag >> 3);
+      if (f <= 9) {
+        if (f != which) { m = ep_wire_fresh(); which = f; }
+        WireReader<kS> s = r;
+        s.end = r.p + len;
+        if (!ep_wire_member(s, which, n, m, deps)) return FPX_ERR_WIRE;
+      }
+      r.p += len;
+    } else if (!r.skip(wt)) {
+      return FPX_ERR_WIRE;
+    }
+  }
+  *kind = which;
+  if (which == 0) return FPX_OK;
+  // "Message missing required fields": the member's, PrepareOk's optional triple aside, and the nested ones
+  const uint32_t roles = ep_wire_roles(which);
+  unsigned need = 0, sub = 0;
+  for (int f = 1; f <= 8; ++f) {
+    const int role = (int)((roles >> (4 * (f - 1))) & 15u);
+    if (role == kEfNone) continue;
+    if (!(which == 8 && f >= 6)) need |= 1u << (f - 1);
+    if (!(m.have >> (f - 1) & 1u)) continue;
+    sub |= role == kEfInstance ? kSubInstance : role == kEfBallot ? kSubBallot : role == kEfVote ? kSubVote
+         : role == kEfDeps ? kSubNumReplicas : 0u;
+  }
+  if ((m.have & need) != need || (m.sub & sub) != sub) return FPX_ERR_WIRE;
+  // parsed, but not a set or status the engine holds
+  if ((sub & kSubNumReplicas) && (m.num_replicas != n || m.dcount != n)) return FPX_ERR_UNSUPPORTED;
+  if (which == 8 && (uint32_t)m.status > 2u) return FPX_ERR_UNSUPPORTED;
+  return FPX_OK;
+}
+
+struct EpWireDecodeParams {
+  const uint8_t* bytes;     // 16-byte aligned
+  const int32_t* offs;      // n + 1
+  int32_t n;
+  int32_t replicas;
+  int32_t value_id_base;
+  int32_t* kind;
+  int32_t* rows;            // n * (12 + replicas)
+  int2* values;             // n {off, len}
+  DevStatus* st;
+  uint32_t* refused;        // the EPaxos handle's refusal word (EpState::refused)
+  uint32_t tag;             // this call's batch tag
+};
+
+// A message that fails refuses the call like a handler's validation pass: the handle's calls queued behind it
+// apply nothing until the status is collected.  Like those passes, it returns at once behind an earlier refusal.
+__global__ void __launch_bounds__(kWireDecThreads) ep_wire_decode_kernel(EpWireDecodeParams P) {
+  {
+    const uint32_t rf = __ldcg(P.refused);
+    if (rf != 0 && rf != P.tag) return;
+  }
+  __shared__ __align__(16) uint8_t s_buf[kWireStage + 32];
+  const int m0 = blockIdx.x * kWireDecThreads;
+  const int m1 = min(P.n, m0 + kWireDecThreads);
+  const WireSpan w = wire_stage_span(P.bytes, P.offs, P.n, m0, m1, s_buf);
+  const int i = m0 + threadIdx.x;
+  if (i >= m1) return;
+  const long long a = P.offs[i], b = P.offs[i + 1];
+  const int n = P.replicas;
+  int32_t* row = P.rows + (long long)i * (EW_DEPS + n);
+  EpWireMsg m = ep_wire_fresh();
+  int kind = 0, code = FPX_ERR_WIRE;
+  if (w.sane && a <= b && a >= w.lo && b <= w.hi) {      // offsets must be monotone
+    if (w.staged) {
+      WireReader<true> r{(uint32_t)__cvta_generic_to_shared(s_buf), nullptr, (uint32_t)(a - w.base), (uint32_t)(b - w.base), true};
+      code = ep_wire_decode_one(r, n, &kind, m, row + EW_DEPS);
+      m.voff += (uint32_t)w.base;                         // window -> buffer offsets
+    } else {
+      WireReader<false> r{0u, P.bytes, (uint32_t)a, (uint32_t)b, true};
+      code = ep_wire_decode_one(r, n, &kind, m, row + EW_DEPS);
+    }
+  }
+  if (code != FPX_OK) {
+    report_error(P.st, code, i);
+    *(volatile uint32_t*)P.refused = P.tag;
+    kind = 0;
+    m = ep_wire_fresh();
+  }
+  const uint32_t roles = ep_wire_roles(kind);
+  bool value = false, deps = false;
+  for (int f = 1; f <= 8; ++f) {
+    if (!(m.have >> (f - 1) & 1u)) continue;
+    const int role = (int)((roles >> (4 * (f - 1))) & 15u);
+    value |= role == kEfValue;
+    deps |= role == kEfDeps;
+  }
+  P.kind[i] = kind;
+  row[EW_IREP] = m.irep; row[EW_INUM] = m.inum; row[EW_BORD] = m.bord; row[EW_BREP] = m.brep;
+  row[EW_REPLICA] = m.replica; row[EW_VBORD] = m.vord; row[EW_VBREP] = m.vrep; row[EW_STATUS] = m.status;
+  row[EW_VALUE] = !value ? -1 : m.noop ? FPX_VALUE_NOOP : P.value_id_base + i;
+  row[EW_SEQ] = m.seq;
+  row[EW_FLAGS] = kind == 8 && (m.have & 0xe0u) == 0xe0u ? 1 : 0;      // PrepareOk's triple is there
+  row[EW_OVERFLOW] = m.overflow;
+  if (!deps)
+    for (int k = 0; k < n; ++k) row[EW_DEPS + k] = 0;
+  P.values[i] = value ? make_int2((int)m.voff, (int)m.vlen) : make_int2(0, 0);
+}
+
+// decoded rows -> the input rows of one handler call (the fpx_epaxos_* layouts); call = FPX_EP_CALL_*
+__host__ __device__ constexpr int ep_wire_pack_kind(int call) {
+  return call == 1 ? 2 : call == 2 ? 4 : call == 3 ? 3 : call == 4 ? 5 : call == 5 ? 6 : call == 6 ? 9 : call == 8 ? 7
+       : call == 9 ? 8 : 0;
+}
+__host__ __device__ constexpr int ep_wire_pack_width(int call, int n) {
+  return call == 1 ? 6 + 2 * n : call == 2 || call == 3 ? 6 + n : call == 4 ? 6 : call == 5 ? 4 + n : call == 9 ? 9 : 4;
+}
+struct EpWirePackParams {
+  int32_t call, replicas;
+  const int32_t* kind;        // [count], the batch's from `first` on
+  const int32_t* rows;        // [count][12 + replicas]
+  int32_t first, count;       // first: error indices are the batch's
+  const int32_t* local_deps;  // [count][replicas] or null (zeros)
+  int32_t* out;               // [count][ep_wire_pack_width]
+  DevStatus* st;
+  uint32_t* refused;
+  uint32_t tag;
+};
+__global__ void __launch_bounds__(256) ep_wire_pack_kernel(EpWirePackParams P) {
+  {
+    const uint32_t rf = __ldcg(P.refused);
+    if (rf != 0 && rf != P.tag) return;
+  }
+  const int j = blockIdx.x * 256 + threadIdx.x;
+  if (j >= P.count) return;
+  const int n = P.replicas, call = P.call;
+  const int32_t* r = P.rows + (long long)j * (EW_DEPS + n);
+  int32_t* o = P.out + (long long)j * ep_wire_pack_width(call, n);
+  int code = FPX_OK;
+  if (P.kind[j] != ep_wire_pack_kind(call)) code = FPX_ERR_INVALID_ARG;
+  // sparse sets (overflow values) the handlers would read: fpx_epaxos_preaccept_sets' rule
+  else if ((call == 1 || call == 2 || call == 3 || call == 5) && r[EW_OVERFLOW] > 0) code = FPX_ERR_UNSUPPORTED;
+  if (code != FPX_OK) {
+    report_error(P.st, code, (long long)P.first + j);
+    *(volatile uint32_t*)P.refused = P.tag;
+    return;
+  }
+  if (call == 5) {                                            // commit {rep, num, value_id, seq, deps}
+    o[0] = r[EW_IREP]; o[1] = r[EW_INUM]; o[2] = r[EW_VALUE]; o[3] = r[EW_SEQ];
+    for (int k = 0; k < n; ++k) o[4 + k] = r[EW_DEPS + k];
+    return;
+  }
+  o[0] = r[EW_IREP]; o[1] = r[EW_INUM]; o[2] = r[EW_BORD]; o[3] = r[EW_BREP];
+  if (call == 1 || call == 2) {                               // {.., value_id, seq, [local_deps,] deps}
+    o[4] = r[EW_VALUE]; o[5] = r[EW_SEQ];
+    int c = 6;
+    if (call == 1) {
+      for (int k = 0; k < n; ++k) o[6 + k] = P.local_deps ? P.local_deps[(long long)j * n + k] : 0;
+      c += n;
+    }
+    for (int k = 0; k < n; ++k) o[c + k] = r[EW_DEPS + k];
+  } else if (call == 3) {                                     // {.., from, seq, deps}
+    o[4] = r[EW_REPLICA]; o[5] = r[EW_SEQ];
+    for (int k = 0; k < n; ++k) o[6 + k] = r[EW_DEPS + k];
+  } else if (call == 4) {                                     // {.., from, 0}
+    o[4] = r[EW_REPLICA]; o[5] = 0;
+  } else if (call == 9) {                                     // {.., from, vb_ord, vb_rep, status, value_id}
+    o[4] = r[EW_REPLICA]; o[5] = r[EW_VBORD]; o[6] = r[EW_VBREP]; o[7] = r[EW_STATUS];
+    o[8] = r[EW_FLAGS] & 1 ? r[EW_VALUE] : 0;                 // a NotSeen vote carries none: 0, as fpx_epaxos_prepare
+  }
 }
 
 // ---------------------------------------------------------------------------
@@ -582,6 +990,222 @@ __global__ void __launch_bounds__(kWireEncThreads) wire_emit_valued_kernel(WireE
       s_dst[slotix] = (uint32_t)(p - P.out);
       s_src[slotix] = m.src;
       s_len[slotix] = vlen;
+    }
+  }
+  if (blockIdx.x == tiles - 1 && threadIdx.x == 0) P.offs[P.n] = (int32_t)(gbase + run);
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int m = warp; m < kWireEncTile; m += kWireEncThreads / 32) {
+    const int len = s_len[m];
+    const uint8_t* src = P.arena + s_src[m];
+    uint8_t* dst = P.out + s_dst[m];
+    for (int k = lane; k < len; k += 32) dst[k] = __ldg(src + k);
+  }
+}
+
+
+// ---------------------------------------------------------------------------
+// EPaxos encoder: one canonical ReplicaInbound per record of a handler call's input and output rows (include/fpx.h
+// fpx_epaxos_wire_encode).  The size -> tile-sum -> emit passes of the gathering encoder above, with a message
+// descriptor of its own: the member's fields in number order by ep_wire_roles, the nested Instance / Ballot /
+// InstancePrefixSetProto written inline, the CommandOrNoop's bytes gathered from the arena by the CTA's warps.
+// ---------------------------------------------------------------------------
+struct EpWireEncodeParams {
+  int32_t call, replicas, self, per_replica;
+  const int32_t* in;          // [n][w_in]   the call's input rows
+  const int32_t* rows;        // [n][w_out]  its replies / events / ballots
+  int32_t w_in, w_out;
+  const int32_t* cmd;         // the handle's cmdLog: value_id of the value-less Commit / Accept records
+  int32_t n;
+  uint8_t* out;
+  int32_t out_capacity;
+  int32_t* offs;              // n + 1
+  uint32_t* tile_sum;
+  const uint8_t* arena;
+  const int32_t* value_offs;
+  int32_t num_values;
+  DevStatus* st;
+  const uint32_t* refused;    // a refused handler call leaves rows unspecified: nothing is encoded behind it
+};
+struct EpMsg {
+  int member;                 // ReplicaInbound field number, 0: a zero-length message
+  unsigned fields;            // bit f - 1: field f of the member is written
+  int irep, inum, bord, brep, vord, vrep, replica, status, seq;
+  const int32_t* deps;        // n watermarks
+  int src, vlen;              // arena[src .. src + vlen)
+  bool noop;
+};
+__device__ __forceinline__ EpMsg ep_enc_msg(const EpWireEncodeParams& P, int i, bool* bad) {
+  EpMsg m{};
+  const int32_t* in = P.in + (long long)i * P.w_in;
+  const int32_t* o = P.rows + (long long)i * P.w_out;
+  m.irep = in[0]; m.inum = in[1];
+  int value = 0;
+  bool cmd_value = false, has_value = false;
+  const int call = P.call, kind = P.w_out ? o[0] : 0;
+  if (call == 0) {                                              // lead -> PreAccept (Replica.scala:697-706)
+    m.member = 2; m.bord = in[2]; m.brep = in[3]; value = in[4]; has_value = true; m.seq = in[5]; m.deps = in + 8;
+  } else if (call == 1 || call == 2) {                          // handlePreAccept / handleAccept replies
+    if (kind == REPLY_OK) {
+      m.member = call == 1 ? 3 : 5; m.bord = o[1]; m.brep = o[2]; m.replica = P.self; m.seq = o[3]; m.deps = o + 4;
+    } else if (kind == REPLY_NACK) {
+      m.member = 9; m.bord = o[1]; m.brep = o[2];
+    } else if (kind == REPLY_COMMIT) {
+      m.member = 6; cmd_value = true; m.seq = o[3]; m.deps = o + 4;
+    } else if (kind != REPLY_NONE) {
+      *bad = true;
+    }
+  } else if (call == 3 || call == 4 || call == 10) {            // PreAcceptOk / AcceptOk / slow-path timer events
+    if (kind == EV_FAST_COMMIT || kind == EV_COMMIT) {
+      m.member = 6; cmd_value = true; m.seq = o[1]; m.deps = o + 2;
+    } else if (kind == EV_SLOW_ACCEPT && call != 4) {
+      m.member = 4; m.bord = in[2]; m.brep = in[3]; cmd_value = true; m.seq = o[1]; m.deps = o + 2;
+    } else if (kind != EV_NONE && !(kind == EV_TIMER && call == 3)) {
+      *bad = true;
+    }
+  } else if (call == 7) {                                       // transitionToPreparePhase -> Prepare
+    m.member = 7; m.bord = o[0]; m.brep = o[1];
+  } else if (call == 8) {                                       // handlePrepare replies
+    if (kind == REPLY_OK) {
+      m.member = 8; m.bord = o[2]; m.brep = o[3]; m.replica = P.self; m.vord = o[4]; m.vrep = o[5]; m.status = o[6];
+      has_value = m.status != ST_NOT_SEEN; value = o[7]; m.seq = o[8]; m.deps = o + 9;
+    } else if (kind == REPLY_NACK) {
+      m.member = 9; m.bord = o[2]; m.brep = o[3];
+    } else if (kind == REPLY_COMMIT) {
+      m.member = 6; has_value = true; value = o[7]; m.seq = o[8]; m.deps = o + 9;
+    } else if (kind != REPLY_NONE) {
+      *bad = true;
+    }
+  }
+  if (!m.member || *bad) { m.member = 0; return m; }
+  m.fields = 0;
+  const uint32_t roles = ep_wire_roles(m.member);
+  for (int f = 1; f <= 8; ++f)
+    if ((roles >> (4 * (f - 1))) & 15u) m.fields |= 1u << (f - 1);
+  if (m.member == 8 && !has_value) m.fields &= 0x1fu;           // NotSeen: no triple (:1655-1744)
+  if (cmd_value) {
+    if ((uint32_t)m.irep >= (uint32_t)P.replicas || (uint32_t)m.inum >= (uint32_t)P.per_replica) { *bad = true; m.member = 0; return m; }
+    value = __ldcg(P.cmd + ((long long)m.inum * P.replicas + m.irep) * kEpCmdWords + C_VALUE);
+    has_value = true;
+  }
+  if (has_value && value == FPX_VALUE_NOOP) {
+    m.noop = true; m.vlen = 2;
+  } else if (has_value) {                                       // value_id v: arena[value_offs[v] .. value_offs[v + 1])
+    if ((uint32_t)value >= (uint32_t)P.num_values) { *bad = true; m.member = 0; return m; }
+    m.src = P.value_offs[value];
+    const long long vl = (long long)P.value_offs[value + 1] - m.src;
+    if (vl < 0) { *bad = true; m.member = 0; return m; }
+    m.vlen = (int)vl;
+  }
+  return m;
+}
+// body bytes of m (kWrite: written at p; *vdst = where the arena's value bytes go, which the caller copies)
+template <bool kWrite>
+__device__ __forceinline__ int ep_msg_body(const EpMsg& m, int n, uint8_t* p, uint8_t** vdst) {
+  const uint32_t roles = ep_wire_roles(m.member);
+  int len = 0;
+  for (int f = 1; f <= 8; ++f) {
+    if (!((m.fields >> (f - 1)) & 1u)) continue;
+    const int role = (int)((roles >> (4 * (f - 1))) & 15u);
+    if (role == kEfInstance || role == kEfBallot || role == kEfVote) {
+      const int a = role == kEfInstance ? m.irep : role == kEfBallot ? m.bord : m.vord;
+      const int b = role == kEfInstance ? m.inum : role == kEfBallot ? m.brep : m.vrep;
+      const int body = 2 + wire_int32_size(a) + wire_int32_size(b);     // <= 22
+      if (kWrite) { *p++ = (uint8_t)(f << 3 | 2); *p++ = (uint8_t)body; p = wire_put_int32(p, 1, a); p = wire_put_int32(p, 2, b); }
+      len += 2 + body;
+    } else if (role >= kEfReplica) {
+      const int v = role == kEfReplica ? m.replica : role == kEfStatus ? m.status : m.seq;
+      len += 1 + wire_int32_size(v);
+      if (kWrite) p = wire_put_int32(p, f, v);
+    } else if (role == kEfValue) {
+      len += 1 + wire_varint_size((unsigned long long)m.vlen) + m.vlen;
+      if (kWrite) {
+        *p++ = (uint8_t)(f << 3 | 2); p = wire_put_varint(p, (unsigned long long)m.vlen);
+        if (m.noop) { *p++ = 0x12; *p++ = 0x00; }                        // CommandOrNoop{noop = 2 {}}
+        else { *vdst = p; p += m.vlen; }
+      }
+    } else {                                                              // InstancePrefixSet.toProto, no values
+      int body = 1 + wire_int32_size(n);
+      for (int k = 0; k < n; ++k) body += 3 + wire_int32_size(m.deps[k]);
+      len += 1 + wire_varint_size((unsigned long long)body) + body;
+      if (kWrite) {
+        *p++ = (uint8_t)(f << 3 | 2); p = wire_put_varint(p, (unsigned long long)body); p = wire_put_int32(p, 1, n);
+        for (int k = 0; k < n; ++k) {
+          const int w = m.deps[k];
+          *p++ = 0x12; *p++ = (uint8_t)(1 + wire_int32_size(w)); p = wire_put_int32(p, 1, w);
+        }
+      }
+    }
+  }
+  return len;
+}
+__device__ __forceinline__ int ep_msg_size(const EpMsg& m, int n) {
+  if (!m.member) return 0;
+  const int b = ep_msg_body<false>(m, n, nullptr, nullptr);
+  return 1 + wire_varint_size((unsigned long long)b) + b;
+}
+
+// pass 1: bytes per tile of kWireEncTile records
+__global__ void __launch_bounds__(kWireEncThreads) ep_wire_size_kernel(EpWireEncodeParams P) {
+  if (__ldcg(P.refused) != 0) return;
+  __shared__ uint32_t s_w[kWireEncThreads / 32];
+  uint32_t sum = 0;
+  int first_bad = INT_MAX;
+  for (int u = 0; u < kWireEncPer; ++u) {
+    const int i = blockIdx.x * kWireEncTile + (int)threadIdx.x * kWireEncPer + u;
+    if (i < P.n) {
+      bool b = false;
+      const EpMsg m = ep_enc_msg(P, i, &b);
+      sum += (uint32_t)ep_msg_size(m, P.replicas);
+      if (b) first_bad = min(first_bad, i);
+    }
+  }
+  if (first_bad != INT_MAX) report_error(P.st, FPX_ERR_INVALID_ARG, first_bad);
+  sum = __reduce_add_sync(0xffffffffu, sum);
+  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = sum;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t t = 0;
+    for (int w = 0; w < kWireEncThreads / 32; ++w) t += s_w[w];
+    P.tile_sum[blockIdx.x] = t;
+  }
+}
+
+// pass 3 (after tile_offsets_kernel): heads by the record's thread, value bytes by the CTA's warps
+__global__ void __launch_bounds__(kWireEncThreads) ep_wire_emit_kernel(EpWireEncodeParams P) {
+  if (__ldcg(P.refused) != 0) return;
+  __shared__ uint32_t s_dst[kWireEncTile];
+  __shared__ int32_t s_src[kWireEncTile], s_len[kWireEncTile];
+  const uint32_t tiles = gridDim.x;
+  if (__ldcg(&P.tile_sum[tiles]) > (uint32_t)P.out_capacity) {   // output buffer too small
+    if (blockIdx.x == 0 && threadIdx.x == 0) report_error(P.st, FPX_ERR_INVALID_ARG, 0);
+    return;
+  }
+  const uint32_t gbase = __ldcg(&P.tile_sum[blockIdx.x]);
+  uint32_t run = 0;
+  for (int u = 0; u < kWireEncPer; ++u) {
+    const int i = blockIdx.x * kWireEncTile + u * kWireEncThreads + threadIdx.x;
+    const int slotix = u * kWireEncThreads + threadIdx.x;
+    bool bad = false;
+    EpMsg m{};
+    if (i < P.n) m = ep_enc_msg(P, i, &bad);
+    const uint32_t sz = i < P.n ? (uint32_t)ep_msg_size(m, P.replicas) : 0u;
+    uint32_t tot;
+    const uint32_t off = run + cta_scan<kWireEncThreads, true>(sz, ScanSum(), &tot);
+    run += tot;
+    s_len[slotix] = 0;
+    if (i < P.n) P.offs[i] = (int32_t)(gbase + off);
+    if (sz) {
+      uint8_t* p = P.out + gbase + off;
+      *p++ = (uint8_t)(m.member << 3 | 2);
+      p = wire_put_varint(p, (unsigned long long)ep_msg_body<false>(m, P.replicas, nullptr, nullptr));
+      uint8_t* vdst = nullptr;
+      ep_msg_body<true>(m, P.replicas, p, &vdst);
+      if (vdst) {
+        s_dst[slotix] = (uint32_t)(vdst - P.out);
+        s_src[slotix] = m.src;
+        s_len[slotix] = m.vlen;
+      }
     }
   }
   if (blockIdx.x == tiles - 1 && threadIdx.x == 0) P.offs[P.n] = (int32_t)(gbase + run);

@@ -16,6 +16,16 @@ EV_RESTART = 1          # prepareok(): run lead(avoid_fast_path = 1) in the retu
 LEADER_NONE, LEADER_PREACCEPTING, LEADER_ACCEPTING, LEADER_PREPARING = 0, 1, 2, 3
 STATUS_NOT_SEEN, STATUS_PRE_ACCEPTED, STATUS_ACCEPTED = 0, 1, 2
 VALUE_NOOP = -(1 << 31)
+# handler calls of the wire codec (include/fpx.h FPX_EP_CALL_*)
+CALL_LEAD, CALL_PREACCEPT, CALL_ACCEPT, CALL_PREACCEPTOK, CALL_ACCEPTOK, CALL_COMMIT, CALL_NACK, CALL_PREPARE_PHASE, \
+    CALL_PREPARE, CALL_PREPAREOK, CALL_SLOW_PATH_TIMER = range(11)
+WIRE_COLS = 12          # a decoded row: 12 + n ints
+
+
+def wire_pack_width(call, n):
+    """ints per row of the handler input that fpx_epaxos_wire_pack writes for `call`"""
+    return {CALL_PREACCEPT: 6 + 2 * n, CALL_ACCEPT: 6 + n, CALL_PREACCEPTOK: 6 + n, CALL_ACCEPTOK: 6,
+            CALL_COMMIT: 4 + n, CALL_NACK: 4, CALL_PREPARE: 4, CALL_PREPAREOK: 9}.get(call, 1)
 
 
 class EpaxosReplica(_Handle):
@@ -128,6 +138,68 @@ class EpaxosReplica(_Handle):
         out = np.zeros((max(len(rows), 1), 4 + self.n), dtype=np.int32)
         self._host_call(self._L.fpx_epaxos_preaccept_sets, rows.ctypes.data, len(rows), oc.ctypes.data, out.ctypes.data)
         return out[:len(rows)]
+
+    # -- wire codec: ReplicaInbound bytes -> handler rows (include/fpx.h, fpx_epaxos_wire_*)
+    def wire_decode(self, buf, offsets, value_id_base=0):
+        """buf: the messages back to back, offsets[m+1] -> (kind[m], rows[m, 12+n], values[m, 2]): kind = the
+        ReplicaInbound member's field number, rows {inst_replica, inst_number, b_ord, b_rep, replica_index, vb_ord,
+        vb_rep, status, value_id, seq, flags, overflow, deps[n]}, values = the CommandOrNoop's {off, len} in buf."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offsets = np.ascontiguousarray(offsets, dtype=np.int32)
+        m = len(offsets) - 1
+        kind = np.zeros(max(m, 1), dtype=np.int32)
+        rows = np.zeros((max(m, 1), WIRE_COLS + self.n), dtype=np.int32)
+        values = np.zeros((max(m, 1), 2), dtype=np.int32)
+        self._host_call(self._L.fpx_epaxos_wire_decode, buf.ctypes.data if len(buf) else None, offsets.ctypes.data, m,
+                        value_id_base, kind.ctypes.data, rows.ctypes.data, values.ctypes.data)
+        return kind[:m], rows[:m], values[:m]
+
+    def wire_pack(self, call, kind, rows, first=0, count=None, local_deps=None):
+        """Decoded rows [first, first+count) -> the input rows of handler call `call` (CALL_*); local_deps [count, n]
+        fills a preaccept row's local columns (zeros if None)."""
+        kind = np.ascontiguousarray(kind, dtype=np.int32)
+        rows = np.ascontiguousarray(rows, dtype=np.int32).reshape(-1, WIRE_COLS + self.n)
+        count = len(rows) - first if count is None else count
+        out = np.zeros((max(count, 1), wire_pack_width(call, self.n)), dtype=np.int32)
+        ld = None if local_deps is None else np.ascontiguousarray(local_deps, dtype=np.int32).reshape(-1, self.n)
+        self._host_call(self._L.fpx_epaxos_wire_pack, call, kind.ctypes.data, rows.ctypes.data, first, count,
+                        None if ld is None else ld.ctypes.data, out.ctypes.data)
+        return out[:count]
+
+    def wire_encode(self, call, in_rows, out_rows=None, arena=None, value_offsets=None):
+        """One canonical ReplicaInbound per record of handler call `call` (its input rows and its replies / events /
+        ballots) -> (bytes, offsets[m+1]); a record with nothing to send is a zero-length message.  value_id v is
+        arena[value_offsets[v] .. value_offsets[v+1]); the value-less Commit / Accept records read the cmdLog."""
+        w_in = {CALL_LEAD: 8 + self.n, CALL_PREACCEPT: 6 + 2 * self.n, CALL_ACCEPT: 6 + self.n,
+                CALL_PREACCEPTOK: 6 + self.n, CALL_ACCEPTOK: 6, CALL_PREPARE_PHASE: 2, CALL_PREPARE: 4,
+                CALL_SLOW_PATH_TIMER: 4}.get(call, 1)
+        in_rows = np.ascontiguousarray(in_rows, dtype=np.int32).reshape(-1, w_in)
+        m = len(in_rows)
+        out_rows = None if out_rows is None else np.ascontiguousarray(out_rows, dtype=np.int32).reshape(m, -1)
+        arena = np.zeros(0, dtype=np.uint8) if arena is None else np.ascontiguousarray(arena, dtype=np.uint8)
+        value_offsets = np.zeros(1, dtype=np.int32) if value_offsets is None else \
+            np.ascontiguousarray(value_offsets, dtype=np.int32)
+        vmax = int(np.diff(value_offsets).max()) if len(value_offsets) > 1 else 2
+        cap = m * (128 + 14 * self.n + max(vmax, 2)) + 16
+        out = np.zeros(cap, dtype=np.uint8)
+        offs = np.zeros(m + 1, dtype=np.int32)
+        self._host_call(self._L.fpx_epaxos_wire_encode, call, in_rows.ctypes.data,
+                        None if out_rows is None else out_rows.ctypes.data, m, arena.ctypes.data if len(arena) else None,
+                        value_offsets.ctypes.data, len(value_offsets) - 1, out.ctypes.data, cap, offs.ctypes.data)
+        return out[:offs[m]].copy(), offs
+
+    def wire_encode_dev(self, call, d_in, d_out_rows, m, d_arena, d_value_offsets, num_values, d_out, out_capacity,
+                        d_offsets):
+        self._check(self._L.fpx_epaxos_wire_encode_dev(self.h, call, d_in, d_out_rows, m, d_arena, d_value_offsets,
+                                                       num_values, d_out, out_capacity, d_offsets))
+
+    def wire_decode_dev(self, d_bytes, d_offsets, m, value_id_base, d_kind, d_rows, d_values):
+        """device pointers, asynchronous on self.stream: a message that fails refuses like a handler batch (sync())"""
+        self._check(self._L.fpx_epaxos_wire_decode_dev(self.h, d_bytes, d_offsets, m, value_id_base, d_kind, d_rows,
+                                                       d_values))
+
+    def wire_pack_dev(self, call, d_kind, d_rows, first, count, d_local_deps, d_out):
+        self._check(self._L.fpx_epaxos_wire_pack_dev(self.h, call, d_kind, d_rows, first, count, d_local_deps, d_out))
 
     def entry(self, rep, num):
         out = np.zeros(7 + self.n, dtype=np.int32)

@@ -636,6 +636,81 @@ float fpx_epaxos_last_kernel_ms(fpx_epaxos* e);
 int fpx_epaxos_entry(fpx_epaxos* e, int32_t inst_replica, int32_t inst_number, int32_t* out,
                      int32_t* leader_kind, int32_t* largest_ballot);
 
+/* ---- Wire codec of EPaxos: ReplicaInbound bytes -> handler rows, on the handle's device and stream ----------
+ * S/epaxos/EPaxos.proto: ReplicaInbound :220-235 {client_request = 1, pre_accept = 2, pre_accept_ok = 3, accept = 4,
+ * accept_ok = 5, commit = 6, prepare = 7, prepare_ok = 8, nack = 9}; Instance :35-41, Ballot :46-52, Command :61-78,
+ * CommandOrNoop :80-88 {command = 1, noop = 2}, CommandStatus :91-95, InstancePrefixSetProto :97-103
+ * {numReplicas = 1, repeated int_prefix_set = 2}, S/compact/IntPrefixSet.proto IntPrefixSetProto {watermark = 1,
+ * repeated value = 2}.  Batches, offsets[n+1], alignment and the parsing rules as for the codec above, and:
+ *   - nested messages are parsed as protobuf-java's mergeFrom builds them: a member, Instance or Ballot given
+ *     again merges into the earlier one (a later scalar wins, a field the second copy lacks keeps its value);
+ *     another member starts afresh.  `required` is checked at every level of the message that results (Command's
+ *     four fields included).  A missing one is FPX_ERR_WIRE at the message's index;
+ *   - `value` is accepted packed and unpacked;
+ *   - a second command_or_noop (or ClientRequest.command) is FPX_ERR_WIRE, as for vanilla Mencius;
+ *   - a dependency set the handle cannot hold -- numReplicas != n, or a count of int_prefix_set entries != n (a
+ *     second `dependencies` concatenates its entries) -- and a PrepareOk status outside {0, 1, 2} are
+ *     FPX_ERR_UNSUPPORTED at that message: scalapb would parse them.
+ * A message that fails stands like a refused batch (see the batch contract above): the fpx_epaxos_*_dev calls
+ * queued behind it apply nothing, and fpx_epaxos_sync reports the status and the first failing index.
+ *
+ * Decode: kind[i] = the member's field number (0: none, or the message failed); rows of 12+n ints
+ *   {inst_replica, inst_number, b_ord, b_rep, replica_index, vb_ord, vb_rep, status, value_id, seq, flags,
+ *    overflow, deps[n]}
+ * Nack's largest_ballot fills b_ord / b_rep.  A pair the message does not carry is (-1, -1), any other column 0
+ * (fpx_epaxos_prepare's convention), value_id -1.  value_id = value_id_base + i for a message carrying a Command
+ * (a CommandOrNoop whose last member is not noop), FPX_VALUE_NOOP for a noop, -1 without a CommandOrNoop.  flags
+ * bit 0: a PrepareOk carries all of its optional command_or_noop, sequence_number and dependencies.  overflow =
+ * number of `value` entries over the message's sets; deps = the n watermarks.  values[i] = {off, len}: the
+ * CommandOrNoop's bytes in the batch ({0, 0} without one); for a ClientRequest the whole `command` field, tag and
+ * length included, which are the bytes of CommandOrNoop().withCommand(command). */
+enum { FPX_EP_CALL_LEAD = 0, FPX_EP_CALL_PREACCEPT = 1, FPX_EP_CALL_ACCEPT = 2, FPX_EP_CALL_PREACCEPTOK = 3,
+       FPX_EP_CALL_ACCEPTOK = 4, FPX_EP_CALL_COMMIT = 5, FPX_EP_CALL_NACK = 6, FPX_EP_CALL_PREPARE_PHASE = 7,
+       FPX_EP_CALL_PREPARE = 8, FPX_EP_CALL_PREPAREOK = 9, FPX_EP_CALL_SLOW_PATH_TIMER = 10 };
+int fpx_epaxos_wire_decode(fpx_epaxos* e, const uint8_t* bytes, const int32_t* offsets, int32_t n,
+                           int32_t value_id_base, int32_t* kind, int32_t* rows, int32_t* values, int64_t* err_index);
+int fpx_epaxos_wire_decode_dev(fpx_epaxos* e, const uint8_t* d_bytes, const int32_t* d_offsets, int32_t n,
+                               int32_t value_id_base, int32_t* d_kind, int32_t* d_rows, int32_t* d_values);
+/* Pack: decoded rows [first, first+count) of a batch (kind and rows are the whole batch's arrays) -> the input
+ * rows of one handler call (FPX_EP_CALL_*): preaccept 6+2n (local_deps, count rows of n ints -- the conflict
+ * index's answers -- fill its local columns, zeros if null), accept 6+n, preacceptok 6+n, acceptok 6, commit 4+n,
+ * nack 4, prepare 4, prepareok 9 (value_id 0 without the triple, as fpx_epaxos_prepare writes).  A row of another
+ * kind is FPX_ERR_INVALID_ARG; a preaccept, accept, preacceptok or commit row with overflow > 0 is
+ * FPX_ERR_UNSUPPORTED (fpx_epaxos_preaccept_sets' rule: parse that set on the host, union with fpx_depset_union).
+ * Error indices are the batch's (first + j); a failing row refuses like a failing message.  Any other call is
+ * FPX_ERR_INVALID_ARG. */
+int fpx_epaxos_wire_pack(fpx_epaxos* e, int32_t call, const int32_t* kind, const int32_t* rows, int32_t first,
+                         int32_t count, const int32_t* local_deps, int32_t* out, int64_t* err_index);
+int fpx_epaxos_wire_pack_dev(fpx_epaxos* e, int32_t call, const int32_t* d_kind, const int32_t* d_rows, int32_t first,
+                             int32_t count, const int32_t* d_local_deps, int32_t* d_out);
+/* Encode: one canonical ReplicaInbound per record of a handler call -- `in` = the call's input rows, `out_rows` =
+ * its replies / events / ballots (unused for lead) -- fields in number order, required fields always, optional ones
+ * when present; a record with nothing to send is a ZERO-LENGTH message.  Per call (Replica.scala):
+ *   lead              PreAccept{instance, ballot, value, seq, deps} (:697-706)
+ *   preaccept         OK PreAcceptOk{instance, reply ballot, replica_index = this replica, seq, deps} (:1279-1288);
+ *                     NACK Nack{instance, largest_ballot}; COMMIT Commit{instance, value, seq, deps} (:1226-1233)
+ *   accept            OK AcceptOk{instance, ballot, replica_index}; NACK; COMMIT (:1455-1510)
+ *   preacceptok,      FAST_COMMIT / COMMIT Commit (:834-845); SLOW_ACCEPT Accept{instance, the row's ballot, value,
+ *   slow_path_timer   seq, deps} (:766-774); TIMER / NONE nothing
+ *   acceptok          COMMIT Commit
+ *   prepare_phase     Prepare{instance, the returned ballot}
+ *   prepare           OK PrepareOk{ballot, instance, replica_index, vote_ballot, status, and command_or_noop,
+ *                     sequence_number, dependencies only when status != NotSeen} (:1655-1744); NACK; COMMIT (:1748-1755)
+ * commit, nack and prepareok send nothing: FPX_ERR_INVALID_ARG.  Values as in the vanilla Mencius encoders (value_id v
+ * = arena[value_offsets[v] .. value_offsets[v+1]), FPX_VALUE_NOOP = 12 00, anything else FPX_ERR_INVALID_ARG at the
+ * record, as is a reply kind the call does not produce).  Dependency sets are written dense: numReplicas = n and n
+ * {watermark} entries (InstancePrefixSet.toProto of an empty-`values` set).  The Commit replies of preaccept and
+ * accept and the Commit / Accept of the events carry no value_id in their rows: the encoder reads the instance's
+ * value_id from the handle's cmdLog.  So encode BEFORE the next call that rewrites those instances; a _dev encode
+ * queued right after its handler on the handle's stream reads that handler's result.  Behind a refused call the
+ * _dev encode writes nothing. */
+int fpx_epaxos_wire_encode(fpx_epaxos* e, int32_t call, const int32_t* in, const int32_t* out_rows, int32_t n,
+                           const uint8_t* arena, const int32_t* value_offsets, int32_t num_values, uint8_t* out,
+                           int32_t out_capacity, int32_t* offsets, int64_t* err_index);
+int fpx_epaxos_wire_encode_dev(fpx_epaxos* e, int32_t call, const int32_t* d_in, const int32_t* d_out_rows, int32_t n,
+                               const uint8_t* d_arena, const int32_t* d_value_offsets, int32_t num_values, uint8_t* d_out,
+                               int32_t out_capacity, int32_t* d_offsets);
+
 /* Batched IntPrefixSet union (S/compact/IntPrefixSet.scala:253-259 == repeated
  * addAll :317-351, then compact :426-431).  Sets in CSR form: watermark[j] and
  * values[off[j] .. off[j+1]) (canonical: every value > its watermark); group q
