@@ -32,6 +32,7 @@
 #include "fpx_tally.cuh"
 #include "fpx_vanilla.cuh"
 #include "fpx_wire.cuh"
+#include "fpx_wire_reads.cuh"
 
 using namespace fpx;
 
@@ -71,6 +72,7 @@ struct fpx_engine {
   // wire codec staging (grown on demand)
   struct WireBuf { void* p = nullptr; size_t cap = 0; };
   WireBuf w_bytes, w_offs, w_kind, w_rec, w_sender, w_out, w_tiles, w_arena, w_voffs;
+  WireBuf w_rw_scratch, w_rw_out;      // the replica decode's per-message and per-tile scratch, its host-form output
   DevStatus* st = nullptr;
   // multi-GPU exchange
   DevExchange* xch = nullptr;          // device copy of the exchange descriptor
@@ -1282,3 +1284,4 @@ int fpx_snapshot_log(fpx_engine* e, int32_t first_slot, int32_t n_slots, int32_t
 #include "fpx_engine_epaxos_wire.inc"
 #include "fpx_engine_f4.inc"
 #include "fpx_engine_reads.inc"
+#include "fpx_engine_wire_reads.inc"

@@ -20,6 +20,8 @@ CHOSEN_RANGE = np.dtype([("slot_start", "<i4"), ("slot_end", "<i4")])
 VM_SKIP = np.dtype([("server", "<i4"), ("slot_start", "<i4"), ("slot_stop", "<i4"), ("own", "<i4")])
 VALUE_NOOP = -(1 << 31)
 WIRE_REC = np.dtype([("a", "<i4"), ("b", "<i4"), ("c", "<i4"), ("d", "<i4")])
+# fpx_read_request: ReadRequest / SequentialReadRequest {slot}; EventualReadRequest: slot = -1
+READ_REQUEST = np.dtype([("slot", "<i4"), ("handle", "<i4")])
 WIRE_PROXYLEADER_INBOUND, WIRE_ACCEPTOR_INBOUND = 0, 1
 WIRE_MENCIUS_PROXYLEADER_INBOUND, WIRE_MENCIUS_ACCEPTOR_INBOUND = 2, 3
 # ServerInbound members (S/vanillamencius/VanillaMencius.proto:227-241): Engine.wire_decode_vm_server_inbound's kinds
@@ -450,6 +452,53 @@ class Engine(_Handle):
 
     def wire_encode_phase2b_dev(self, d_in, n, d_out, out_capacity, d_offsets):
         self._check(self._L.fpx_wire_encode_phase2b_dev(self.h, d_in, n, d_out, out_capacity, d_offsets))
+
+    # -- MultiPaxos replica and acceptor read-path wire codec (include/fpx.h)
+    def wire_decode_replica_inbound(self, buf, offsets, value_id_base=0, handle_base=0, reads_capacity=None):
+        """ReplicaInbound bytes -> (kind[n], chosen, chosen_values[k, 2], reads, read_commands[k, 2], split): records
+        of the messages [0, split) only; continue with offsets[split:].  reads_capacity defaults to a bound no batch
+        can exceed: a Command field takes at least 12 bytes (tag, length, command_id with its three required fields,
+        command)."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offsets = np.ascontiguousarray(offsets, dtype=np.int32)
+        n = len(offsets) - 1
+        cap = int(offsets[-1] - offsets[0]) // 12 + 1 if reads_capacity is None else reads_capacity
+        kind = np.zeros(max(n, 1), dtype=np.int32)
+        chosen = np.zeros(max(n, 1), dtype=CHOSEN)
+        cvals = np.zeros((max(n, 1), 2), dtype=np.int32)
+        reads = np.zeros(max(cap, 1), dtype=READ_REQUEST)
+        rcmds = np.zeros((max(cap, 1), 2), dtype=np.int32)
+        counts = np.zeros(3, dtype=np.int32)
+        self._host_call(self._L.fpx_wire_decode_replica_inbound, buf.ctypes.data if len(buf) else None,
+                        offsets.ctypes.data, n, value_id_base, handle_base, cap, kind.ctypes.data, chosen.ctypes.data,
+                        cvals.ctypes.data, reads.ctypes.data, rcmds.ctypes.data, counts.ctypes.data)
+        nc, nr, split = (int(x) for x in counts)
+        return kind[:n], chosen[:nc].copy(), cvals[:nc].copy(), reads[:nr].copy(), rcmds[:nr].copy(), split
+
+    def wire_encode_max_slot_replies(self, buf, kind, recs):
+        """The acceptor's MaxSlotReply / BatchMaxSlotReply per decoded AcceptorInbound record (a = group << 16 |
+        acceptor, b = maxVotedSlot) of the request batch buf -> (bytes, offsets[n+1])."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        kind = np.ascontiguousarray(kind, dtype=np.int32)
+        recs = np.ascontiguousarray(recs, dtype=WIRE_REC)
+        # a reply is at most 64 bytes of heads plus the request body's client_address
+        cap = int(64 * len(recs) + np.where((kind == 3) | (kind == 4), recs["d"], 0).clip(0).sum()) + 16
+        n = len(recs)
+        out = np.zeros(cap, dtype=np.uint8)
+        offs = np.zeros(n + 1, dtype=np.int32)
+        self._host_call(self._L.fpx_wire_encode_max_slot_replies, buf.ctypes.data if len(buf) else None, len(buf),
+                        kind.ctypes.data, recs.ctypes.data, n, out.ctypes.data, cap, offs.ctypes.data)
+        return out[:offs[n]].copy(), offs
+
+    def wire_decode_replica_inbound_dev(self, d_bytes, d_offsets, n, value_id_base, handle_base, reads_capacity, d_kind,
+                                        d_chosen, d_chosen_values, d_reads, d_read_commands, d_counts):
+        self._check(self._L.fpx_wire_decode_replica_inbound_dev(self.h, d_bytes, d_offsets, n, value_id_base, handle_base,
+                                                                reads_capacity, d_kind, d_chosen, d_chosen_values,
+                                                                d_reads, d_read_commands, d_counts))
+
+    def wire_encode_max_slot_replies_dev(self, d_bytes, n_bytes, d_kind, d_in, n, d_out, out_capacity, d_offsets):
+        self._check(self._L.fpx_wire_encode_max_slot_replies_dev(self.h, d_bytes, n_bytes, d_kind, d_in, n, d_out,
+                                                                 out_capacity, d_offsets))
 
     # -- device-pointer calls (raw device addresses, asynchronous on self.stream)
     def proxyleader_arm_dev(self, d_in, n):

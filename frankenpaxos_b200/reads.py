@@ -8,15 +8,13 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .engine import _Handle
+from .engine import READ_REQUEST, _Handle
 
 READS_CLIENT, READS_READ_BATCHER = 0, 1
 READ_OPEN = np.dtype([("key", "<i4"), ("id", "<i4")])
 # MaxSlotReply / BatchMaxSlotReply with the read's key; voter = group << 16 | acceptor
 MAX_SLOT_REPLY = np.dtype([("key", "<i4"), ("id", "<i4"), ("voter", "<i4"), ("slot", "<i4")])
 READ_SLOT = np.dtype([("key", "<i4"), ("id", "<i4"), ("slot", "<i4"), ("reserved", "<i4")])
-# ReadRequest / SequentialReadRequest {slot}; EventualReadRequest: slot = -1
-READ_REQUEST = np.dtype([("slot", "<i4"), ("handle", "<i4")])
 READ_REPLY = np.dtype([("handle", "<i4"), ("reply_slot", "<i4"), ("after_slot", "<i4"), ("reserved", "<i4")])
 
 
@@ -69,6 +67,45 @@ class Reads(_Handle):
 
     def advance_dev(self, d_watermark, d_out):
         self._check(self._L.fpx_reads_advance_dev(self.h, d_watermark, d_out))
+
+    # -- wire codec (include/fpx.h fpx_reads_wire_*)
+    def wire_decode(self, buf, offsets):
+        """ClientInbound (READS_CLIENT) or ReadBatcherInbound (READS_READ_BATCHER) bytes -> (kind[n],
+        MAX_SLOT_REPLY[n], spans[n, 2]); a record of another member has key -1, which the tally ignores."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offsets = np.ascontiguousarray(offsets, dtype=np.int32)
+        n = len(offsets) - 1
+        kind = np.zeros(max(n, 1), dtype=np.int32)
+        out = np.zeros(max(n, 1), dtype=MAX_SLOT_REPLY)
+        spans = np.zeros((max(n, 1), 2), dtype=np.int32)
+        self._host_call(self._L.fpx_reads_wire_decode, buf.ctypes.data if len(buf) else None, offsets.ctypes.data, n,
+                        kind.ctypes.data, out.ctypes.data, spans.ctypes.data)
+        return kind[:n], out[:n], spans[:n]
+
+    def wire_encode_read_requests(self, recs, arena, value_offsets):
+        """READ_SLOT records of completed reads -> (bytes, offsets[n+1]): ReadRequest (Client) or ReadRequestBatch
+        (ReadBatcher); arena entry `key` is the message's command field(s), tag and length included."""
+        recs = np.ascontiguousarray(recs, dtype=READ_SLOT)
+        arena = np.ascontiguousarray(arena, dtype=np.uint8)
+        value_offsets = np.ascontiguousarray(value_offsets, dtype=np.int32)
+        n = len(recs)
+        lens = np.diff(value_offsets)
+        ok = (recs["key"] >= 0) & (recs["key"] < len(lens))
+        cap = int(17 * n + lens[recs["key"][ok]].sum()) + 16    # tag, length (<= 5) and slot (<= 11) per message
+        out = np.zeros(cap, dtype=np.uint8)
+        offs = np.zeros(n + 1, dtype=np.int32)
+        self._host_call(self._L.fpx_reads_wire_encode_read_requests, recs.ctypes.data, n,
+                        arena.ctypes.data if len(arena) else None, value_offsets.ctypes.data, len(value_offsets) - 1,
+                        out.ctypes.data, cap, offs.ctypes.data)
+        return out[:offs[n]].copy(), offs
+
+    def wire_decode_dev(self, d_bytes, d_offsets, n, d_kind, d_out, d_spans):
+        self._check(self._L.fpx_reads_wire_decode_dev(self.h, d_bytes, d_offsets, n, d_kind, d_out, d_spans))
+
+    def wire_encode_read_requests_dev(self, d_in, n, d_arena, d_value_offsets, num_values, d_out, out_capacity,
+                                      d_offsets):
+        self._check(self._L.fpx_reads_wire_encode_read_requests_dev(self.h, d_in, n, d_arena, d_value_offsets,
+                                                                    num_values, d_out, out_capacity, d_offsets))
 
     def sync(self, check=True):
         r = _lib.ReadsSyncResult()

@@ -988,6 +988,86 @@ typedef struct {
 } fpx_reads_sync_result;
 int fpx_reads_sync(fpx_reads* r, fpx_reads_sync_result* out);
 
+/* ---- Wire codec of the MultiPaxos replica and read path (S/multipaxos/MultiPaxos.proto) --------------------
+ * ClientInbound :489-500, ReadBatcherInbound :513-523, AcceptorInbound :551-561, ReplicaInbound :563-576,
+ * CommandId :188-196, Command :198-204, MaxSlotRequest / MaxSlotReply :316-331, BatchMaxSlotRequest /
+ * BatchMaxSlotReply :333-349, the read requests :351-396.  Parsing rules, offsets[n+1] batches, 16-byte aligned
+ * buffers of the _dev forms and canonical output as for the wire codec above.  A member given more than once,
+ * a Command and a CommandId are merged as protobuf-java's mergeFrom builds them (have-bits accumulate, a later
+ * scalar wins, a repeated field appends), and `required` is checked on the merged message at every level.  A
+ * malformed message or a missing required field is FPX_ERR_WIRE at the message's index.  The _dev forms run on
+ * the engine's stream; their status and first index are collected by fpx_sync (engine calls) or fpx_reads_sync
+ * (fpx_reads calls).  The fpx_reads calls stage through their engine's buffers.
+ *
+ * fpx_wire_decode_replica_inbound (protocol FPX_MULTIPAXOS, else FPX_ERR_UNSUPPORTED): kind[i] = the member's
+ * field number (0: none, no record).  Records only for the messages [0, split), where split is the index of the
+ * first read message (kinds 2..7) that follows a Chosen in the batch, or n:
+ *   1 chosen  -> chosen[k] = {slot, value_id_base + i}, dense in delivery order, and chosen_values[2k..2k+1] =
+ *                {off, len} of the CommandBatchOrNoop (located, not parsed; a second one is FPX_ERR_WIRE).  The
+ *                records go to fpx_replica_chosen[_dev] as they are.
+ *   2..7      -> reads[k] = {slot, handle_base + k} per Command, dense in delivery order, a batch's Commands in
+ *                wire order; read_commands[2k..2k+1] = {off, len} of the Command message (its body: what
+ *                Command.parseFrom takes).  Eventual reads (4, 7) get slot = -1.  A second `command` in a
+ *                read_request, sequential_read_request or eventual_read_request is FPX_ERR_WIRE (protobuf would
+ *                merge the two Commands).  More records than reads_capacity: FPX_ERR_OVERFLOW_FULL at the first
+ *                message whose Commands do not fit.
+ * counts = {n_chosen, n_reads, split} (_dev: a device int32[3] written on the stream).  The order of the batch is
+ * the reference's when the caller runs fpx_reads_replica(reads), fpx_replica_chosen(chosen), then
+ * fpx_reads_advance(the new watermark), and continues with the messages from offsets + split (value_id_base and
+ * handle_base advanced by what it has used).  After an error the records and counts are unspecified. */
+int fpx_wire_decode_replica_inbound(fpx_engine* e, const uint8_t* bytes, const int32_t* offsets, int32_t n,
+                                    int32_t value_id_base, int32_t handle_base, int32_t reads_capacity, int32_t* kind,
+                                    fpx_chosen* chosen, int32_t* chosen_values, fpx_read_request* reads,
+                                    int32_t* read_commands, int32_t* counts, int64_t* err_index);
+int fpx_wire_decode_replica_inbound_dev(fpx_engine* e, const uint8_t* d_bytes, const int32_t* d_offsets, int32_t n,
+                                        int32_t value_id_base, int32_t handle_base, int32_t reads_capacity,
+                                        int32_t* d_kind, fpx_chosen* d_chosen, int32_t* d_chosen_values,
+                                        fpx_read_request* d_reads, int32_t* d_read_commands, int32_t* d_counts);
+/* The acceptor's answers (Acceptor.scala:222-254): kind[] and in[] as fpx_wire_decode_inbound(
+ * FPX_WIRE_ACCEPTOR_INBOUND) writes them for the request batch bytes[0 .. n_bytes), with a = group << 16 |
+ * acceptor and b = maxVotedSlot filled in by the caller (fpx_snapshot_acceptor(..., n_slots = 0) at the request's
+ * batch boundary).  One message per record:
+ *   3 max_slot_request       -> ClientInbound{max_slot_reply{command_id, group_index, acceptor_index, slot}}; the
+ *                               request's CommandId merged and written canonically, client_address copied;
+ *   4 batch_max_slot_request -> ReadBatcherInbound{batch_max_slot_reply{read_batcher_index, read_batcher_id,
+ *                               acceptor_index, slot}};
+ *   any other kind           -> a zero-length message.
+ * A body that does not parse or lacks a required field is FPX_ERR_WIRE at its record; a voter that names no
+ * acceptor of the config is FPX_ERR_INVALID_ARG. */
+int fpx_wire_encode_max_slot_replies(fpx_engine* e, const uint8_t* bytes, int32_t n_bytes, const int32_t* kind,
+                                     const fpx_wire_rec* in, int32_t n, uint8_t* out, int32_t out_capacity,
+                                     int32_t* offsets, int64_t* err_index);
+int fpx_wire_encode_max_slot_replies_dev(fpx_engine* e, const uint8_t* d_bytes, int32_t n_bytes, const int32_t* d_kind,
+                                         const fpx_wire_rec* d_in, int32_t n, uint8_t* d_out, int32_t out_capacity,
+                                         int32_t* d_offsets);
+/* The replies a Client or ReadBatcher receives, by the handle's kind; out[] goes to fpx_reads_max_slot_replies[_dev]
+ * as it is, spans[2i..2i+1] = {off, len} of the member's body (its last occurrence), {0, 0} for no member.
+ *   FPX_READS_CLIENT, ClientInbound: max_slot_reply (4) -> {key = client_pseudonym, id = client_id,
+ *     voter = group_index << 16 | acceptor_index, slot} (Client.scala:851-931 keys by pseudonym and checks only the
+ *     clientId; client_address is required but not compared).
+ *   FPX_READS_READ_BATCHER, ReadBatcherInbound: batch_max_slot_reply (4) -> {key = floorMod(read_batcher_id,
+ *     key_capacity), id = read_batcher_id, voter = acceptor_index, slot} (ReadBatcher.scala:568-623;
+ *     read_batcher_index is required but not used).  fpx_reads_open must open read_batcher_id under that key
+ *     for the replies to find their read; the primer's id -1 is key key_capacity - 1.
+ *   A group_index or acceptor_index outside [0, 2^15) gives voter = -1 (FPX_ERR_BAD_ACCEPTOR if counted).
+ *   Every other member (replies, read replies, NotLeader, ...) gets key = -1, which the tally ignores, and is
+ *   not parsed: the host reads it from its span. */
+int fpx_reads_wire_decode(fpx_reads* r, const uint8_t* bytes, const int32_t* offsets, int32_t n, int32_t* kind,
+                          fpx_max_slot_reply* out, int32_t* spans, int64_t* err_index);
+int fpx_reads_wire_decode_dev(fpx_reads* r, const uint8_t* d_bytes, const int32_t* d_offsets, int32_t n, int32_t* d_kind,
+                              fpx_max_slot_reply* d_out, int32_t* d_spans);
+/* One canonical ReplicaInbound per completed read (fpx_read_slot of the tally): read_request{slot, command} for the
+ * Client (Client.scala:900-911), read_request_batch{slot, command*} for the ReadBatcher (ReadBatcher.scala:613-617).
+ * Value id = the record's key: arena[value_offsets[key] .. value_offsets[key+1]) is the message's `command`
+ * field or fields, tag and length included (12 len Command, repeated for a batch).  A key outside
+ * [0, num_values) is FPX_ERR_INVALID_ARG at its record. */
+int fpx_reads_wire_encode_read_requests(fpx_reads* r, const fpx_read_slot* in, int32_t n, const uint8_t* arena,
+                                        const int32_t* value_offsets, int32_t num_values, uint8_t* out,
+                                        int32_t out_capacity, int32_t* offsets, int64_t* err_index);
+int fpx_reads_wire_encode_read_requests_dev(fpx_reads* r, const fpx_read_slot* d_in, int32_t n, const uint8_t* d_arena,
+                                            const int32_t* d_value_offsets, int32_t num_values, uint8_t* d_out,
+                                            int32_t out_capacity, int32_t* d_offsets);
+
 /* The engine's CUDA stream (a cudaStream_t) so a caller can order its own work
  * (events, NCCL collectives) with the engine's. */
 void* fpx_stream(fpx_engine* e);
