@@ -411,7 +411,12 @@ int fpx_wire_decode_inbound_dev(fpx_engine* e, int32_t inbound, const uint8_t* d
                                 int32_t n, int32_t* d_kind, fpx_wire_rec* d_out);
 /* ProxyLeaderInbound{phase2b}: the acceptor's replies, ready for transport.send.  offsets[n+1]
  * is written; the bytes must fit out_capacity (FPX_ERR_INVALID_ARG otherwise).  With protocol
- * FPX_MENCIUS the mencius shape is written ({acceptor_index, slot, round} under field 4). */
+ * FPX_MENCIUS the mencius shape is written ({acceptor_index, slot, round} under field 4).
+ * out_capacity, for every encoder of this header: output that does not fit is refused with
+ * FPX_ERR_INVALID_ARG at index 0.  Then nothing at or past out[out_capacity] is written, the host
+ * forms leave the caller's out untouched, and the contents of a _dev form's d_out below
+ * out_capacity are unspecified (the small-record encoders write the tiles that fit, the others
+ * nothing).  The refusal latches nothing: the handle's next call runs as usual. */
 int fpx_wire_encode_phase2b(fpx_engine* e, const fpx_p2b* in, int32_t n, uint8_t* out, int32_t out_capacity,
                             int32_t* offsets, int64_t* err_index);
 int fpx_wire_encode_phase2b_dev(fpx_engine* e, const fpx_p2b* d_in, int32_t n, uint8_t* d_out, int32_t out_capacity,

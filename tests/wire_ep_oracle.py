@@ -324,9 +324,17 @@ def inbound_message(G, call, r, n):
     return m.SerializeToString()
 
 
-def expected_encode(G, call, in_rows, out_rows, n, me, cmd_value):
+def expected_encode(G, call, in_rows, out_rows, n, me, cmd_value, entries=None):
     """SerializeToString of what the reference sends for each record (include/fpx.h fpx_epaxos_wire_encode);
-    cmd_value(rep, num) = the instance's value_id in the replica's cmdLog"""
+    cmd_value(rep, num) = the instance's value_id in the replica's cmdLog.  entries: value_id v is the CommandOrNoop
+    whose bytes are entries[v] (None: value_arena's values)"""
+    def put(field, v):
+        if entries is None or v == VALUE_NOOP:
+            _set_value(G, field, v)
+        else:
+            field.SetInParent()
+            field.MergeFromString(entries[v])
+
     out = []
     for i, r in enumerate(np.asarray(in_rows).tolist()):
         o = [] if out_rows is None else [int(x) for x in out_rows[i]]
@@ -335,14 +343,14 @@ def expected_encode(G, call, in_rows, out_rows, n, me, cmd_value):
 
         def commit(v, seq, deps):
             b = m.commit
-            _set_value(G, b.command_or_noop, v); b.sequence_number = seq; _set_deps(G, b.dependencies, deps)
+            put(b.command_or_noop, v); b.sequence_number = seq; _set_deps(G, b.dependencies, deps)
             return b
 
         b = None
         if call == CALL_LEAD:
             b = m.pre_accept
             b.ballot.ordering, b.ballot.replica_index = r[2], r[3]
-            _set_value(G, b.command_or_noop, r[4]); b.sequence_number = r[5]; _set_deps(G, b.dependencies, r[8:8 + n])
+            put(b.command_or_noop, r[4]); b.sequence_number = r[5]; _set_deps(G, b.dependencies, r[8:8 + n])
         elif call in (CALL_PREACCEPT, CALL_ACCEPT):
             if o[0] == 1 and call == CALL_PREACCEPT:
                 b = m.pre_accept_ok
@@ -363,7 +371,7 @@ def expected_encode(G, call, in_rows, out_rows, n, me, cmd_value):
             elif o[0] == 2:
                 b = m.accept
                 b.ballot.ordering, b.ballot.replica_index = r[2], r[3]
-                _set_value(G, b.command_or_noop, cmd_value(*inst)); b.sequence_number = o[1]
+                put(b.command_or_noop, cmd_value(*inst)); b.sequence_number = o[1]
                 _set_deps(G, b.dependencies, o[2:2 + n])
         elif call == CALL_PREPARE_PHASE:
             b = m.prepare
@@ -376,7 +384,7 @@ def expected_encode(G, call, in_rows, out_rows, n, me, cmd_value):
                 b.vote_ballot.ordering, b.vote_ballot.replica_index = o[4], o[5]
                 b.status = o[6]
                 if o[6]:
-                    _set_value(G, b.command_or_noop, o[7]); b.sequence_number = o[8]
+                    put(b.command_or_noop, o[7]); b.sequence_number = o[8]
                     _set_deps(G, b.dependencies, o[9:9 + n])
             elif o[0] == 2:
                 b = m.nack
