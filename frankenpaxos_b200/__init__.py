@@ -8,7 +8,7 @@ does -- there is no CPU fallback.
 """
 from .engine import (CHOSEN, NACK, P2A, P2B, Engine, FpxError, dst,  # noqa: F401
                      MULTIPAXOS, MENCIUS, VANILLA_MENCIUS, VM_REPLY_PHASE2B, VM_REPLY_NACK, VM_REPLY_CHOSEN,
-                     VM_REPLY_CHOSEN_RETIRED, P2A_RANGE, P2B_RANGE, CHOSEN_RANGE, VM_SKIP, VALUE_NOOP,
+                     VM_REPLY_CHOSEN_RETIRED, P2A_RANGE, P2B_RANGE, CHOSEN_RANGE, MENCIUS_CHOSEN, VM_SKIP, VALUE_NOOP,
                      WIRE_REC, WIRE_PROXYLEADER_INBOUND, WIRE_ACCEPTOR_INBOUND,
                      WIRE_MENCIUS_PROXYLEADER_INBOUND, WIRE_MENCIUS_ACCEPTOR_INBOUND, VM_WIRE_CLIENT_REQUEST,
                      VM_WIRE_PHASE2A, VM_WIRE_PHASE2B, VM_WIRE_SKIP, VM_WIRE_CHOSEN, VM_WIRE_PHASE2_NACK)

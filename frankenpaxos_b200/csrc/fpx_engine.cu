@@ -67,6 +67,7 @@ struct fpx_engine {
   int32_t* rng_dec = nullptr;              // per-record scratch of the range kernels (FPX_MAX_RANGE_BATCH)
   uint32_t rng_seq_base = 1;               // Phase2bNoopRange delivery sequence numbers
   int unit_ranges = 0;                     // a one-slot range was ever armed: arms must look at the range keys
+  int32_t* mix = nullptr;                  // mencius: scratch of the mixed replica call (fpx_mencius_replica_inbound)
   // fpx_step_dev: CUDA events around the acceptor and tally kernels of the last kStepRing steps
   std::vector<cudaEvent_t> step_ev;        // [kStepRing][4], created on first use
   // wire codec staging (grown on demand)
@@ -371,6 +372,9 @@ int fpx_create(fpx_engine** out, const fpx_config* cfg) {
     e->rng_cap = std::max(1024, g.ovf_cap);
     CK(e, R.alloc(&e->rng_tab, (size_t)e->rng_cap * kRangeWords * 4));
     CK(e, R.alloc(&e->rng_tab_spare, (size_t)e->rng_cap * kRangeWords * 4));
+    // fpx_mencius_replica_inbound: {split, ranges, -, -}, the ranges' indices, the per-tile counts
+    const size_t tiles = ((size_t)cfg->max_batch + kMixTile - 1) / kMixTile;
+    CK(e, R.alloc(&e->mix, (4 + (size_t)FPX_MAX_RANGE_BATCH + tiles + 1) * 4));
   }
   if (cfg->protocol != FPX_MULTIPAXOS) CK(e, R.alloc(&e->rng_dec, (size_t)(FPX_MAX_RANGE_BATCH + 1) * 4));
   CK(e, R.alloc(&e->st, sizeof(DevStatus)));

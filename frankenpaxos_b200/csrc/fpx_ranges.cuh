@@ -366,6 +366,13 @@ __global__ void renormalize_range_stamps_kernel(RangeTable t) {
 // record that is already in the log (min-reduce), then the put-if-absent fill below it.
 // Batch contract (FPX_ERR_BATCH_ORDER): two records of one call must not cover a common
 // slot -- the second one's stop position would depend on the first one's progress.
+//
+// kMixed: the same two passes over the multi-slot records of a mixed Chosen / ChosenNoopRange batch
+// (fpx_mencius_replica_inbound, below), one CTA row per listed record in turn.  Their one-slot records have been
+// put into the log first, each under its own delivery number seq_base + i (first one wins, as in handleChosen), so a
+// range of index j stops at its first slot whose entry is older than seq_base + j: put before the call, or by a
+// one-slot record delivered before the range.  Its fill then replaces the entries of later one-slot records below
+// that stop (atomicMin of the smaller delivery number), which the reference would have found taken.
 // ---------------------------------------------------------------------------
 struct ReplicaRangeParams {
   Geometry g;
@@ -373,18 +380,23 @@ struct ReplicaRangeParams {
   int32_t n;
   uint32_t seq_base;
   unsigned long long* rlog;
-  int32_t* first;    // [n], preset to kNoHit
+  int32_t* first;    // [n], preset to kNoHit (kMixed: [listed records])
   DevStatus* st;
+  // kMixed: fpx_mencius_chosen records, the listed multi-slot records' indices and the call's control words
+  const int4* in4;
+  const int32_t* list;
+  const int32_t* ctl;
 };
 
-__global__ void __launch_bounds__(256) replica_range_first_kernel(ReplicaRangeParams P) {
+// kMixed: rows of the list that are applied (listed and before the split)
+__device__ __forceinline__ int mixed_listed(const ReplicaRangeParams& P) {
+  return min(__ldcg(&P.ctl[1]), (int)FPX_MAX_RANGE_BATCH);
+}
+
+// one record's first hit: the first slot of rec = [start, end) that is already in the log -> first[y]
+template <bool kMixed>
+__device__ __forceinline__ void replica_range_first_one(const ReplicaRangeParams& P, int y, int j, int2 rec) {
   const Geometry& g = P.g;
-  const int j = blockIdx.y;
-  const int2 rec = P.in[j];
-  if (range_precheck(g, rec.x, rec.y, 0) != FPX_OK) {
-    if (blockIdx.x == 0 && threadIdx.x == 0) report_error(P.st, FPX_ERR_SLOT_RANGE, j);
-    return;
-  }
   const long long LG = g.lgroups;
   const long long count = (rec.y - rec.x + LG - 1) / LG;
   int hit = kNoHit;
@@ -393,19 +405,22 @@ __global__ void __launch_bounds__(256) replica_range_first_kernel(ReplicaRangePa
     int slot = (int)(rec.x + t * LG);
     int l = local_slot(g, slot);
     // ascending per thread: first hit is its minimum.  A retired slot is in the log (executed long ago).
-    if (l == kLocalRetired || (l >= 0 && __ldcg(&P.rlog[l]) != kU64Empty)) hit = slot;
+    if (kMixed) {   // an empty entry reads as delivery number 0xffffffff: never older than seq_base + j
+      if (l == kLocalRetired || (l >= 0 && (uint32_t)(__ldcg(&P.rlog[l]) >> 32) < P.seq_base + (uint32_t)j)) hit = slot;
+    } else {
+      if (l == kLocalRetired || (l >= 0 && __ldcg(&P.rlog[l]) != kU64Empty)) hit = slot;
+    }
   }
   hit = __reduce_min_sync(0xffffffffu, hit);
-  if ((threadIdx.x & 31) == 0 && hit != kNoHit) atomicMin(&P.first[j], hit);
+  if ((threadIdx.x & 31) == 0 && hit != kNoHit) atomicMin(&P.first[y], hit);
 }
 
-__global__ void __launch_bounds__(256) replica_range_fill_kernel(ReplicaRangeParams P) {
+// one record's fill below min(end, first[y]); returns the largest ordinal this thread put
+template <bool kMixed>
+__device__ __forceinline__ int replica_range_fill_one(const ReplicaRangeParams& P, int y, int j, int2 rec) {
   const Geometry& g = P.g;
-  const int j = blockIdx.y;
-  const int2 rec = P.in[j];
-  if (range_precheck(g, rec.x, rec.y, 0) != FPX_OK) return;
   const long long LG = g.lgroups;
-  const int stop = min(rec.y, __ldcg(&P.first[j]));
+  const int stop = min(rec.y, __ldcg(&P.first[y]));
   const long long count = stop > rec.x ? (stop - rec.x + LG - 1) / LG : 0;
   int mx = INT_MIN;
   for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < count; t += (long long)gridDim.x * blockDim.x) {
@@ -413,9 +428,182 @@ __global__ void __launch_bounds__(256) replica_range_fill_kernel(ReplicaRangePar
     if (l < 0) continue;
     unsigned long long old = atomicMin(&P.rlog[l], ((unsigned long long)(P.seq_base + (uint32_t)j) << 32) |
                                                        (uint32_t)FPX_VALUE_NOOP);
-    if (old != kU64Empty)   // another record of this call covers the slot too: the later of the two is at fault
+    // another record of this call covers the slot too: the later of the two is at fault.  (kMixed: only a later
+    // one-slot record can be there, and the range is right to take the slot from it.)
+    if (!kMixed && old != kU64Empty)
       report_error(P.st, FPX_ERR_BATCH_ORDER, max((long long)j, (long long)(uint32_t)(old >> 32) - (long long)P.seq_base));
     mx = max(mx, g.base_local + ring_to_rel(g, l));   // an ordinal, like every other writer of max_chosen_local
+  }
+  return mx;
+}
+
+// kMixed: the listed record of row y (y < rows), or false at the first one at or past the split
+__device__ __forceinline__ bool mixed_listed_rec(const ReplicaRangeParams& P, int y, int* j, int2* rec) {
+  *j = __ldg(&P.list[y]);
+  if (*j >= __ldcg(&P.ctl[0])) return false;      // the list is in delivery order
+  const int4 r = __ldg(&P.in4[*j]);
+  *rec = make_int2(r.x, r.y);
+  return true;
+}
+
+template <bool kMixed>
+__global__ void __launch_bounds__(256) replica_range_first_kernel(ReplicaRangeParams P) {
+  if (!kMixed) {
+    const int j = blockIdx.y;
+    const int2 rec = P.in[j];
+    if (range_precheck(P.g, rec.x, rec.y, 0) != FPX_OK) {
+      if (blockIdx.x == 0 && threadIdx.x == 0) report_error(P.st, FPX_ERR_SLOT_RANGE, j);
+      return;
+    }
+    replica_range_first_one<false>(P, j, j, rec);
+    return;
+  }
+  const int rows = mixed_listed(P);
+  for (int y = blockIdx.y; y < rows; y += gridDim.y) {
+    int j;
+    int2 rec;
+    if (!mixed_listed_rec(P, y, &j, &rec)) break;
+    replica_range_first_one<true>(P, y, j, rec);
+  }
+}
+
+template <bool kMixed>
+__global__ void __launch_bounds__(256) replica_range_fill_kernel(ReplicaRangeParams P) {
+  int mx = INT_MIN;
+  if (!kMixed) {
+    const int j = blockIdx.y;
+    const int2 rec = P.in[j];
+    if (range_precheck(P.g, rec.x, rec.y, 0) != FPX_OK) return;
+    mx = replica_range_fill_one<false>(P, j, j, rec);
+  } else {
+    const int rows = mixed_listed(P);
+    for (int y = blockIdx.y; y < rows; y += gridDim.y) {
+      int j;
+      int2 rec;
+      if (!mixed_listed_rec(P, y, &j, &rec)) break;
+      mx = max(mx, replica_range_fill_one<true>(P, y, j, rec));
+    }
+  }
+  mx = __reduce_max_sync(0xffffffffu, mx);
+  if ((threadIdx.x & 31) == 0 && mx != INT_MIN) atomicMax(&P.st->max_chosen_local, mx);
+}
+
+// ---------------------------------------------------------------------------
+// A mixed batch of the replica's Chosen and ChosenNoopRange messages in delivery order (fpx_mencius_replica_inbound):
+// record {s, e, v} stands for the slots s, s + LG, ... < e.  Replica.handleChosen (S/mencius/Replica.scala:402-420)
+// and handleChosenNoopRange (:464-486) are both "put v into the slots until the first one already in the log", so a
+// record of one slot is a put-if-absent and only the records of two or more slots ("ranges") can stop part way.
+// The call applies the records before `split`, the smallest of
+//   (a) the first range that shares a slot with an earlier range (full extents): its stop would depend on that
+//       range's progress;
+//   (b) the first range past FPX_MAX_RANGE_BATCH;
+// and n.  Passes: mixed_count -> tile_offsets -> mixed_list (the ranges in delivery order, rule (b)) ->
+// mixed_overlap (rule (a)) -> mixed_single (the one-slot records, statuses) -> replica_range_first / _fill<true>.
+// ctl = {split, ranges}.
+// ---------------------------------------------------------------------------
+constexpr int kMixPer = 4, kMixThreads = 256, kMixTile = kMixPer * kMixThreads;
+
+struct MixedParams {
+  Geometry g;
+  const int4* in;
+  int32_t n;
+  uint32_t seq_base;
+  unsigned long long* rlog;
+  uint32_t* tile;     // [tiles] ranges per tile, then their exclusive offsets
+  int32_t* list;      // [FPX_MAX_RANGE_BATCH] the ranges' record indices, delivery order
+  int32_t* first;     // [FPX_MAX_RANGE_BATCH] their stops, preset to kNoHit
+  int32_t* ctl;       // {split, ranges}
+  DevStatus* st;
+};
+
+// slots the record covers (0 for a record that fails range_precheck)
+__device__ __forceinline__ long long mixed_count(const Geometry& g, int4 r) {
+  if (range_precheck(g, r.x, r.y, 0) != FPX_OK) return 0;
+  return (r.y - (long long)r.x + g.lgroups - 1) / g.lgroups;
+}
+
+__global__ void __launch_bounds__(kMixThreads) mixed_count_kernel(MixedParams P) {
+  uint32_t c = 0;
+  for (int u = 0; u < kMixPer; ++u) {
+    const int i = blockIdx.x * kMixTile + (int)threadIdx.x * kMixPer + u;
+    if (i < P.n) c += mixed_count(P.g, __ldg(&P.in[i])) >= 2;
+  }
+  c = cta_reduce<kMixThreads>(c, ScanSum());
+  if (threadIdx.x == 0) P.tile[blockIdx.x] = c;
+  if (blockIdx.x == 0 && threadIdx.x == 0) P.ctl[0] = P.n;
+}
+
+__global__ void __launch_bounds__(kMixThreads) mixed_list_kernel(MixedParams P) {
+  bool multi[kMixPer];
+  uint32_t c = 0;
+  const int i0 = blockIdx.x * kMixTile + (int)threadIdx.x * kMixPer;
+#pragma unroll
+  for (int u = 0; u < kMixPer; ++u) {
+    multi[u] = i0 + u < P.n && mixed_count(P.g, __ldg(&P.in[i0 + u])) >= 2;
+    c += multi[u];
+  }
+  uint32_t rank = __ldcg(&P.tile[blockIdx.x]) + cta_scan<kMixThreads, true>(c, ScanSum());
+#pragma unroll
+  for (int u = 0; u < kMixPer; ++u) {
+    if (!multi[u]) continue;
+    if (rank < (uint32_t)FPX_MAX_RANGE_BATCH) {
+      P.list[rank] = i0 + u;
+      P.first[rank] = kNoHit;
+    } else if (rank == (uint32_t)FPX_MAX_RANGE_BATCH) {
+      atomicMin(&P.ctl[0], i0 + u);                 // rule (b)
+    }
+    ++rank;
+  }
+}
+
+// Rule (a) over the listed ranges: every pair (p < q) of ranks, by 256 x 256 tiles of pairs claimed in turn by a
+// fixed grid.  Two ranges share a slot iff they start in the same residue mod LG and max(starts) < min(ends).
+__global__ void __launch_bounds__(kMixThreads) mixed_overlap_kernel(MixedParams P) {
+  __shared__ int s_s[kMixThreads], s_e[kMixThreads];
+  const int K = min(__ldcg(&P.ctl[1]), (int)FPX_MAX_RANGE_BATCH);
+  const long long T = (K + kMixThreads - 1) / kMixThreads;
+  const int LG = P.g.lgroups;
+  for (long long t = blockIdx.x; t < T * (T + 1) / 2; t += gridDim.x) {
+    // t -> (q, p), p <= q: t = q (q + 1) / 2 + p
+    long long q = (long long)((sqrt(8.0 * (double)t + 1.0) - 1.0) / 2.0);
+    while (q * (q + 1) / 2 > t) --q;
+    while ((q + 1) * (q + 2) / 2 <= t) ++q;
+    const long long p = t - q * (q + 1) / 2;
+    const int rp = (int)p * kMixThreads + threadIdx.x, rq = (int)q * kMixThreads + threadIdx.x;
+    __syncthreads();
+    if (rp < K) {
+      const int4 r = __ldg(&P.in[__ldcg(&P.list[rp])]);
+      s_s[threadIdx.x] = r.x; s_e[threadIdx.x] = r.y;
+    }
+    __syncthreads();
+    if (rq >= K) continue;
+    const int j = __ldcg(&P.list[rq]);
+    const int4 r = __ldg(&P.in[j]);
+    const int res = r.x % LG;
+    const int hi = min(kMixThreads, p == q ? (int)threadIdx.x : K - (int)p * kMixThreads);
+    bool hit = false;
+    for (int k = 0; k < hi; ++k) {
+      const int s = s_s[k];
+      hit |= s % LG == res && max(s, r.x) < min(s_e[k], r.y);
+    }
+    if (hit) atomicMin(&P.ctl[0], j);
+  }
+}
+
+// The one-slot records before the split: put-if-absent under their delivery number (the smallest wins), like
+// replica_chosen_kernel; and the statuses of every record before the split.
+__global__ void __launch_bounds__(kMixThreads) mixed_single_kernel(MixedParams P) {
+  const Geometry& g = P.g;
+  const int split = __ldcg(&P.ctl[0]);
+  int mx = INT_MIN;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < split; i += gridDim.x * blockDim.x) {
+    const int4 r = __ldg(&P.in[i]);
+    if (range_precheck(g, r.x, r.y, 0) != FPX_OK) { report_error(P.st, FPX_ERR_SLOT_RANGE, i); continue; }
+    if (mixed_count(g, r) != 1) continue;
+    const int l = local_slot(g, r.x);
+    if (l < 0) continue;                                   // retired: in the log already (range_precheck bounds it)
+    red_min_u64(&P.rlog[l], ((unsigned long long)(P.seq_base + (uint32_t)i) << 32) | (uint32_t)r.z);
+    mx = max(mx, g.base_local + ring_to_rel(g, l));
   }
   mx = __reduce_max_sync(0xffffffffu, mx);
   if ((threadIdx.x & 31) == 0 && mx != INT_MIN) atomicMax(&P.st->max_chosen_local, mx);

@@ -16,6 +16,9 @@
 // Skip :164-172, Phase2b :174-181, Chosen :183-190, Phase2Nack :209-215) goes through the same
 // kernels: one more inbound of the decoder, Skip through the small-record encoder, and the reply
 // stream, Chosen and Phase2a through the value-gathering one.
+// Compartmentalized Mencius' replica (S/mencius/Mencius.proto: ReplicaInbound :363-371, Chosen :189-195,
+// ChosenNoopRange :197-203) is the decoder's sixth inbound; its Phase2bNoopRange (:178-187), ChosenNoopRange and
+// LeaderInbound.nack = 7 (:322-337) go through the small-record encoder.
 // Parsing rules restated from the published proto2 wire format (DESIGN.md, wire codec): base-128
 // varints of at most 10 bytes, int32 = low 32 bits, unknown fields skipped by wire type, a known
 // number with another wire type is unknown, oneof = last member on the wire, a missing
@@ -32,7 +35,7 @@ constexpr int kWireDecThreads = 256;
 constexpr int kWireEncPer = 4;            // replies per thread of the encoders
 constexpr int kWireEncThreads = 256;
 constexpr int kWireEncTile = kWireEncPer * kWireEncThreads;
-constexpr int kWireMaxP2b = 46, kWireMaxNack = 13;
+constexpr int kWireMaxP2b = 46, kWireMaxNack = 13, kWireMaxP2bRange = 57, kWireMaxChosenRange = 24;
 
 // Byte reader over one message.  kShared: positions index the CTA's staged window in shared memory
 // (explicit ld.shared: a generic pointer would cost a generic load per byte); else they are offsets
@@ -111,10 +114,16 @@ struct WireReader {
 //   inbound 3  mencius AcceptorInbound       (:352-361)                  phase2a = 2, phase2a_noop_range = 3
 //   inbound 4  vanillamencius ServerInbound  (VanillaMencius.proto:227-241)  client_request = 1, phase2a = 4,
 //                                            phase2b = 5, skip = 6, chosen = 7, phase2_nack = 9 (of 9 members)
+//   inbound 5  mencius ReplicaInbound        (Mencius.proto:363-371)     chosen = 1, chosen_noop_range = 2
 enum WireMember { kWmOpaque = 0, kWmP2a, kWmP2b4, kWmRange3, kWmMenciusP2b, kWmRangeVote5, kWmVmRequest, kWmVmP2a,
-                  kWmVmChosen, kWmVmNack };
-template <bool kVm>
+                  kWmVmChosen, kWmVmNack, kWmMrChosen, kWmRange2 };
+// the decoder's instantiations: inbounds 0-3 (chosen at run time), 4, 5
+enum { kWireInPath = 0, kWireInVm = 1, kWireInMenciusReplica = 2 };
+template <int kIn>
 __device__ __forceinline__ int wire_member(int inbound, int which) {
+  constexpr bool kVm = kIn == kWireInVm;
+  if (kIn == kWireInMenciusReplica)   // Chosen {slot, command_batch_or_noop}, ChosenNoopRange {start, end}
+    return which == 1 ? kWmMrChosen : kWmRange2;
   if (kVm)   // vanilla Mencius: Phase2b {server_index, slot, round} has the mencius Phase2b's shape, Skip {server_index,
              // start, stop} that of a noop range
     return which == 1 ? kWmVmRequest : which == 4 ? kWmVmP2a : which == 5 ? kWmMenciusP2b : which == 6 ? kWmRange3
@@ -132,10 +141,12 @@ __device__ __forceinline__ int wire_member_count(int inbound) { return inbound =
 
 // Reader positions in, reader positions out (*value_pos: out->z is a position the caller rebases).
 // *sender: the server field of a vanilla Mencius Phase2a, Phase2b or Skip (their field 1), else -1.
-// kVm: inbound 4 (the only one with a bool, a sender or a ClientRequest span: the other inbounds compile without them)
-template <bool kShared, bool kVm>
+// kIn == kWireInVm: inbound 4 (the only one with a bool, a sender or a ClientRequest span: the other inbounds compile
+// without them); kWireInMenciusReplica: inbound 5, {slot, 0, value_off, value_len} or {start, end, 0, 0}.
+template <bool kShared, int kIn>
 __device__ __forceinline__ bool wire_decode_one(int inbound, int lgroups, int agroups, WireReader<kShared> r, int* kind,
                                                 int4* out, bool* value_pos, int* sender) {
+  constexpr bool kVm = kIn == kWireInVm, kMr = kIn == kWireInMenciusReplica;
   int which = 0;
   uint32_t blo = 0, bhi = 0;
   while (!r.done()) {
@@ -147,7 +158,7 @@ __device__ __forceinline__ bool wire_decode_one(int inbound, int lgroups, int ag
       if (!r.ok || r.end - r.p < n) return false;
       // oneof: the last member wins; a field number the message does not declare is an unknown field: skipped,
       // the earlier member stays (scalapb parseFrom)
-      if ((tag >> 3) <= (uint32_t)(kVm ? 9 : wire_member_count(inbound))) { which = (int)(tag >> 3); blo = r.p; bhi = r.p + n; }
+      if ((tag >> 3) <= (uint32_t)(kVm ? 9 : kMr ? 2 : wire_member_count(inbound))) { which = (int)(tag >> 3); blo = r.p; bhi = r.p + n; }
       r.p += n;
     } else if (!r.skip(wt)) {
       return false;
@@ -158,16 +169,18 @@ __device__ __forceinline__ bool wire_decode_one(int inbound, int lgroups, int ag
   *value_pos = false;
   *sender = -1;
   if (which == 0) return true;
-  const int mk = wire_member<kVm>(inbound, which);
+  const int mk = wire_member<kIn>(inbound, which);
   if (mk == kWmOpaque) {
     *out = make_int4(0, 0, (int)blo, (int)(bhi - blo));
     *value_pos = true;
     return true;
   }
-  const int n_ints = kVm ? (mk == kWmVmRequest ? 0 : mk == kWmVmChosen ? 1 : mk == kWmVmNack ? 2 : 3)
+  const int n_ints = kMr ? (mk == kWmMrChosen ? 1 : 2)
+                   : kVm ? (mk == kWmVmRequest ? 0 : mk == kWmVmChosen ? 1 : mk == kWmVmNack ? 2 : 3)
                          : (mk == kWmP2a ? 2 : mk == kWmP2b4 ? 4 : mk == kWmRangeVote5 ? 5 : 3);
   // the value's field number (0: none) and the required bool's (Chosen.isRevocation)
-  const int vfield = kVm ? (mk == kWmVmP2a ? 4 : mk == kWmVmChosen ? 2 : mk == kWmVmRequest ? 1 : 0) : (mk == kWmP2a ? 3 : 0);
+  const int vfield = kMr ? (mk == kWmMrChosen ? 2 : 0)
+                   : kVm ? (mk == kWmVmP2a ? 4 : mk == kWmVmChosen ? 2 : mk == kWmVmRequest ? 1 : 0) : (mk == kWmP2a ? 3 : 0);
   const int bfield = kVm && mk == kWmVmChosen ? 3 : 0;
   WireReader<kShared> b = r;
   b.p = blo; b.end = bhi; b.ok = true;
@@ -202,6 +215,11 @@ __device__ __forceinline__ bool wire_decode_one(int inbound, int lgroups, int ag
   }
   // "Message missing required fields."
   if (have != (1u << n_ints) - 1u || (vfield && !have_value) || (bfield && !have_bool)) return false;
+  if (kMr) {
+    if (mk == kWmMrChosen) { *out = make_int4(v0, 0, (int)off, (int)len); *value_pos = true; }
+    else *out = make_int4(v0, v1, 0, 0);
+    return true;
+  }
   if (kVm) {
     if (mk == kWmVmP2a || mk == kWmMenciusP2b || mk == kWmRange3) *sender = v0;
     if (mk == kWmVmP2a) { *out = make_int4(v1, v2, (int)off, (int)len); *value_pos = true; return true; }
@@ -232,6 +250,9 @@ struct WireDecodeParams {
   int4* out;
   int32_t* sender;          // vanilla Mencius only (else null): the message's server field, -1 if none
   DevStatus* st;
+  // mencius ReplicaInbound only: out holds fpx_mencius_chosen rows, values[i] the Chosen value's {off, len}
+  int32_t value_id_base;
+  int2* values;
 };
 
 // The byte span of a decoder CTA's messages [m0, m1): staged in s_buf (kWireStage + 32 bytes) when it fits,
@@ -262,11 +283,12 @@ __device__ __forceinline__ WireSpan wire_stage_span(const uint8_t* bytes, const 
   return w;
 }
 
-// kVm: the vanilla Mencius instantiation (inbound 4); the other inbounds' instantiation compiles without its bool,
-// sender and ClientRequest span
-template <bool kVm>
+// kIn: kWireInPath (inbounds 0-3), kWireInVm (the vanilla Mencius inbound 4: the other instantiations compile without
+// its bool, sender and ClientRequest span) or kWireInMenciusReplica (inbound 5: dense fpx_mencius_chosen rows)
+template <int kIn>
 __global__ void __launch_bounds__(kWireDecThreads) wire_decode_kernel(WireDecodeParams P) {
-  const int inbound = kVm ? 4 : P.inbound;
+  constexpr bool kVm = kIn == kWireInVm, kMr = kIn == kWireInMenciusReplica;
+  const int inbound = kVm ? 4 : kMr ? 5 : P.inbound;
   __shared__ __align__(16) uint8_t s_buf[kWireStage + 32];
   const int m0 = blockIdx.x * kWireDecThreads;
   const int m1 = min(P.n, m0 + kWireDecThreads);
@@ -283,14 +305,30 @@ __global__ void __launch_bounds__(kWireDecThreads) wire_decode_kernel(WireDecode
     bool value_pos = false;
     if (staged) {
       WireReader<true> r{(uint32_t)__cvta_generic_to_shared(s_buf), nullptr, (uint32_t)(a - base), (uint32_t)(b - base), true};
-      ok = wire_decode_one<true, kVm>(inbound, P.lgroups, P.agroups, r, &kind, &rec, &value_pos, &sender);
+      ok = wire_decode_one<true, kIn>(inbound, P.lgroups, P.agroups, r, &kind, &rec, &value_pos, &sender);
       if (ok && value_pos) rec.z += (int)base;                  // window -> buffer offsets
     } else {
       WireReader<false> r{0u, P.bytes, (uint32_t)a, (uint32_t)b, true};
-      ok = wire_decode_one<false, kVm>(inbound, P.lgroups, P.agroups, r, &kind, &rec, &value_pos, &sender);
+      ok = wire_decode_one<false, kIn>(inbound, P.lgroups, P.agroups, r, &kind, &rec, &value_pos, &sender);
     }
   }
   if (!ok) report_error(P.st, FPX_ERR_WIRE, i);
+  if (kMr) {
+    // Chosen(slot, v) -> {slot, slot + 1, value_id_base + i}, ChosenNoopRange(s, e) -> {s, e, Noop}; no member (or a
+    // failed message) -> a row that covers no slot
+    int4 row = make_int4(0, 0, FPX_VALUE_NOOP, 0);
+    int2 val = make_int2(0, 0);
+    if (ok && kind == 1) {
+      row = make_int4(rec.x, (int)((uint32_t)rec.x + 1u), P.value_id_base + i, 0);
+      val = make_int2(rec.z, rec.w);
+    } else if (ok && kind == 2) {
+      row = make_int4(rec.x, rec.y, FPX_VALUE_NOOP, 0);
+    }
+    P.kind[i] = ok ? kind : 0;
+    P.out[i] = row;
+    P.values[i] = val;
+    return;
+  }
   P.kind[i] = kind;
   P.out[i] = rec;
   if (kVm) P.sender[i] = ok ? sender : -1;
@@ -724,8 +762,15 @@ __device__ __forceinline__ uint8_t* wire_put_int32(uint8_t* p, int field, int v)
 
 // kWireVm*: vanilla Mencius ServerInbound (VanillaMencius.proto:227-241).  kWireVmReply is the dense reply
 // stream of fpx_vm_phase2a (fpx_p2b {kind, server, slot, round|value}), one message per record by its kind.
+// kWireMencius{Nack, P2bRange, ChosenRange}: compartmentalized Mencius (Mencius.proto) LeaderInbound.nack = 7,
+// ProxyLeaderInbound.phase2b_noop_range = 5 and ReplicaInbound.chosen_noop_range = 2.
 enum { kWirePhase2b = 0, kWireNack = 1, kWireChosen = 2, kWireMenciusPhase2b = 3, kWireVmReply = 4, kWireVmChosen = 5,
-       kWireVmPhase2a = 6, kWireVmSkip = 7 };
+       kWireVmPhase2a = 6, kWireVmSkip = 7, kWireMenciusNack = 8, kWireMenciusP2bRange = 9, kWireMenciusChosenRange = 10 };
+// the largest message of a small-record encoder (its shared-memory slot per record)
+__host__ __device__ constexpr int wire_small_max(int kind) {
+  return kind == kWireNack || kind == kWireMenciusNack ? kWireMaxNack : kind == kWireMenciusP2bRange ? kWireMaxP2bRange
+       : kind == kWireMenciusChosenRange ? kWireMaxChosenRange : kWireMaxP2b;
+}
 // encoders whose messages carry a value from the arena: size -> scan -> wire_emit_valued_kernel
 __host__ __device__ constexpr bool wire_gathers(int kind) {
   return kind == kWireChosen || kind == kWireVmReply || kind == kWireVmChosen || kind == kWireVmPhase2a;
@@ -744,6 +789,7 @@ struct WireEncodeParams {
   int32_t num_values;
   int32_t servers;            // kWireVmPhase2a: sending_server = slot mod servers
   DevStatus* st;
+  int32_t agroups;            // kWireMenciusP2bRange: acceptor_group_index = (dst >> 16) mod agroups
 };
 
 // One message of a value-gathering encoder: outer oneof tag, int32 fields 1..nf, then (vfield != 0) the
@@ -832,6 +878,17 @@ __device__ __forceinline__ int wire_size_of(const WireEncodeParams& P, int i, bo
   } else if (KIND == kWireNack) {
     int2 r = ((const int2*)P.in)[i];
     return 2 + 1 + wire_int32_size(r.y);     // LeaderInbound{nack = 6 {round = 1}}
+  } else if (KIND == kWireMenciusNack) {
+    int2 r = ((const int2*)P.in)[i];
+    return 2 + 1 + wire_int32_size(r.y);     // mencius LeaderInbound{nack = 7 {round = 1}}
+  } else if (KIND == kWireMenciusP2bRange) {
+    int4 r = ((const int4*)P.in)[i];
+    // ProxyLeaderInbound{phase2b_noop_range = 5 {acceptor_group_index, acceptor_index, start, end, round}}
+    return 2 + 5 + wire_int32_size((r.x >> 16) % P.agroups) + wire_int32_size(r.x & 0xffff) + wire_int32_size(r.y) +
+           wire_int32_size(r.z) + wire_int32_size(r.w);
+  } else if (KIND == kWireMenciusChosenRange) {
+    int2 r = ((const int2*)P.in)[i];
+    return 2 + 2 + wire_int32_size(r.x) + wire_int32_size(r.y);   // ReplicaInbound{chosen_noop_range = 2 {start, end}}
   } else {
     const WireMsg m = wire_msg<KIND>(P, i, bad);
     return *bad ? 0 : wire_msg_size(m);
@@ -876,6 +933,7 @@ __global__ void __launch_bounds__(kWireEncThreads) wire_emit_small_kernel(WireEn
   const int i0 = tile * kWireEncTile + (int)threadIdx.x * kWireEncPer;
   int4 rec[kWireEncPer];
   uint32_t sz[kWireEncPer];
+  int rnd[kWireEncPer];       // kWireMenciusP2bRange: the fifth field
   uint32_t mine = 0;
 #pragma unroll
   for (int u = 0; u < kWireEncPer; ++u) {
@@ -893,6 +951,16 @@ __global__ void __launch_bounds__(kWireEncThreads) wire_emit_small_kernel(WireEn
       } else if (KIND == kWireVmSkip) {
         rec[u] = __ldcg((const int4*)P.in + i);
         sz[u] = 2 + 3 + wire_int32_size(rec[u].x) + wire_int32_size(rec[u].y) + wire_int32_size(rec[u].z);
+      } else if (KIND == kWireMenciusP2bRange) {
+        const int4 r = __ldcg((const int4*)P.in + i);
+        rec[u] = make_int4((r.x >> 16) % P.agroups, r.x & 0xffff, r.y, r.z);   // fields 1-4; the round is field 5
+        sz[u] = 2 + 5 + wire_int32_size(rec[u].x) + wire_int32_size(rec[u].y) + wire_int32_size(rec[u].z) +
+                wire_int32_size(rec[u].w) + wire_int32_size(r.w);
+        rnd[u] = r.w;
+      } else if (KIND == kWireMenciusChosenRange) {
+        const int2 r = __ldcg((const int2*)P.in + i);
+        rec[u] = make_int4(r.x, r.y, 0, 0);
+        sz[u] = 2 + 2 + wire_int32_size(r.x) + wire_int32_size(r.y);
       } else {
         int2 r = __ldcg((const int2*)P.in + i);
         rec[u].y = r.y;
@@ -929,6 +997,16 @@ __global__ void __launch_bounds__(kWireEncThreads) wire_emit_small_kernel(WireEn
     } else if (KIND == kWireVmSkip) {
       *p++ = 0x32; *p++ = (uint8_t)(sz[u] - 2);
       p = wire_put_int32(p, 1, rec[u].x); p = wire_put_int32(p, 2, rec[u].y); p = wire_put_int32(p, 3, rec[u].z);
+    } else if (KIND == kWireMenciusP2bRange) {
+      *p++ = 0x2a; *p++ = (uint8_t)(sz[u] - 2);
+      p = wire_put_int32(p, 1, rec[u].x); p = wire_put_int32(p, 2, rec[u].y); p = wire_put_int32(p, 3, rec[u].z);
+      p = wire_put_int32(p, 4, rec[u].w); p = wire_put_int32(p, 5, rnd[u]);
+    } else if (KIND == kWireMenciusChosenRange) {
+      *p++ = 0x12; *p++ = (uint8_t)(sz[u] - 2);
+      p = wire_put_int32(p, 1, rec[u].x); p = wire_put_int32(p, 2, rec[u].y);
+    } else if (KIND == kWireMenciusNack) {
+      *p++ = 0x3a; *p++ = (uint8_t)(sz[u] - 2);
+      p = wire_put_int32(p, 1, rec[u].y);
     } else {
       *p++ = 0x32; *p++ = (uint8_t)(sz[u] - 2);
       p = wire_put_int32(p, 1, rec[u].y);

@@ -18,6 +18,8 @@ P2A_RANGE = np.dtype([("slot_start", "<i4"), ("slot_end", "<i4"), ("round", "<i4
 P2B_RANGE = np.dtype([("dst", "<i4"), ("slot_start", "<i4"), ("slot_end", "<i4"), ("round", "<i4")])
 CHOSEN_RANGE = np.dtype([("slot_start", "<i4"), ("slot_end", "<i4")])
 VM_SKIP = np.dtype([("server", "<i4"), ("slot_start", "<i4"), ("slot_stop", "<i4"), ("own", "<i4")])
+# fpx_mencius_chosen: one message of the Mencius replica's mixed Chosen / ChosenNoopRange stream
+MENCIUS_CHOSEN = np.dtype([("slot_start", "<i4"), ("slot_end", "<i4"), ("value_id", "<i4"), ("reserved", "<i4")])
 VALUE_NOOP = -(1 << 31)
 WIRE_REC = np.dtype([("a", "<i4"), ("b", "<i4"), ("c", "<i4"), ("d", "<i4")])
 # fpx_read_request: ReadRequest / SequentialReadRequest {slot}; EventualReadRequest: slot = -1
@@ -323,6 +325,17 @@ class Engine(_Handle):
         recs = np.ascontiguousarray(recs, dtype=CHOSEN_RANGE)
         self._host_call(self._L.fpx_mencius_replica_chosen_range, recs.ctypes.data, len(recs))
 
+    def mencius_replica_inbound(self, recs):
+        """A mixed Chosen / ChosenNoopRange batch (MENCIUS_CHOSEN records) in delivery order: applies the records before
+        the returned split, as the reference's replica would one at a time; continue with recs[split:]."""
+        recs = np.ascontiguousarray(recs, dtype=MENCIUS_CHOSEN)
+        split = C.c_int32(0)
+        self._host_call(self._L.fpx_mencius_replica_inbound, recs.ctypes.data, len(recs), C.byref(split))
+        return split.value
+
+    def mencius_replica_inbound_dev(self, d_in, n, d_split):
+        self._check(self._L.fpx_mencius_replica_inbound_dev(self.h, d_in, n, d_split))
+
     RANGE_NO_HIT = 0x7f7f7f7f
 
     def mencius_replica_range_first(self, recs):
@@ -375,6 +388,38 @@ class Engine(_Handle):
         cap = int(24 * len(recs) + lens[recs["value_id"][ok]].sum()) + 16
         return self._wire_encode(self._L.fpx_wire_encode_chosen, recs, CHOSEN, 0, arena.ctypes.data if len(arena) else None,
                                  value_offsets.ctypes.data, len(value_offsets) - 1, cap)
+
+    # -- Compartmentalized Mencius noop-range and replica wire codec (protocol=MENCIUS, include/fpx.h)
+    def wire_decode_mencius_replica_inbound(self, buf, offsets, value_id_base=0):
+        """ReplicaInbound bytes -> (kind[n], recs[n] MENCIUS_CHOSEN, values[n, 2]): row i answers message i; values[i]
+        = {off, len} of a Chosen's command_batch_or_noop.  kind 0 (no member) is a row that covers no slot."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offsets = np.ascontiguousarray(offsets, dtype=np.int32)
+        n = len(offsets) - 1
+        kind = np.zeros(max(n, 1), dtype=np.int32)
+        recs = np.zeros(max(n, 1), dtype=MENCIUS_CHOSEN)
+        values = np.zeros((max(n, 1), 2), dtype=np.int32)
+        self._host_call(self._L.fpx_wire_decode_mencius_replica_inbound, buf.ctypes.data if len(buf) else None,
+                        offsets.ctypes.data, n, value_id_base, kind.ctypes.data, recs.ctypes.data, values.ctypes.data)
+        return kind[:n], recs[:n], values[:n]
+
+    def wire_decode_mencius_replica_inbound_dev(self, d_bytes, d_offsets, n, value_id_base, d_kind, d_recs, d_values):
+        self._check(self._L.fpx_wire_decode_mencius_replica_inbound_dev(self.h, d_bytes, d_offsets, n, value_id_base,
+                                                                        d_kind, d_recs, d_values))
+
+    def wire_encode_mencius_phase2b_range(self, recs):
+        """fpx_mencius_acceptor_noop_range's replies -> ProxyLeaderInbound.phase2b_noop_range bytes, offsets[n+1]."""
+        return self._wire_encode(self._L.fpx_wire_encode_mencius_phase2b_range, recs, P2B_RANGE, 57)
+
+    def wire_encode_mencius_chosen_range(self, recs):
+        """fpx_mencius_range_phase2b's ChosenNoopRanges -> ReplicaInbound.chosen_noop_range bytes, offsets[n+1]."""
+        return self._wire_encode(self._L.fpx_wire_encode_mencius_chosen_range, recs, CHOSEN_RANGE, 24)
+
+    def wire_encode_mencius_phase2b_range_dev(self, d_in, n, d_out, out_capacity, d_offsets):
+        self._check(self._L.fpx_wire_encode_mencius_phase2b_range_dev(self.h, d_in, n, d_out, out_capacity, d_offsets))
+
+    def wire_encode_mencius_chosen_range_dev(self, d_in, n, d_out, out_capacity, d_offsets):
+        self._check(self._L.fpx_wire_encode_mencius_chosen_range_dev(self.h, d_in, n, d_out, out_capacity, d_offsets))
 
     # -- vanilla Mencius wire codec (protocol=VANILLA_MENCIUS): ServerInbound bytes <-> records (include/fpx.h)
     def wire_decode_vm_server_inbound(self, buf, offsets):

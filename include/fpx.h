@@ -73,6 +73,10 @@ typedef struct { int32_t slot_start, slot_end, round, dst; } fpx_p2a_range;
 typedef struct { int32_t dst, slot_start, slot_end, round; } fpx_p2b_range;
 /* ChosenNoopRange{slotStartInclusive, slotEndExclusive}. */
 typedef struct { int32_t slot_start, slot_end; } fpx_chosen_range;
+/* One message of the Mencius replica's mixed stream (fpx_mencius_replica_inbound): the slots
+ * slot_start, slot_start + num_leader_groups, ... < slot_end get value_id.  Chosen(slot, v) is
+ * {slot, slot + 1, v}, ChosenNoopRange(s, e) is {s, e, FPX_VALUE_NOOP}; reserved is ignored. */
+typedef struct { int32_t slot_start, slot_end, value_id, reserved; } fpx_mencius_chosen;
 /* S/vanillamencius Skip{serverIndex, startSlotInclusive, stopSlotExclusive} applied to
  * server `server`'s log; own = 1: the fill advanceWithSkips does at the skipping server. */
 typedef struct { int32_t server, slot_start, slot_stop, own; } fpx_vm_skip_rec;
@@ -375,6 +379,26 @@ int fpx_mencius_replica_range_first(fpx_engine* e, const fpx_chosen_range* in, i
                                     int64_t* err_index);
 int fpx_mencius_replica_range_fill(fpx_engine* e, const fpx_chosen_range* in, int32_t n, const int32_t* first,
                                    int64_t* err_index);
+/* Replica.handleChosen (S/mencius/Replica.scala:402-420) and handleChosenNoopRange (:464-486) for ONE batch of both,
+ * in delivery order (fpx_mencius_chosen records, e.g. from fpx_wire_decode_mencius_replica_inbound).  Records
+ * [0, *split) are applied exactly as the reference applies those messages one at a time: each record puts its value
+ * into its slots until the first slot already in the log -- put before the call, retired by fpx_retire_below, or put
+ * by an earlier record of the call -- and stops there.  A record of one slot is therefore handleChosen's
+ * put-if-absent (the first Chosen of a slot wins), a record covering no slot changes nothing.  Records of two or more
+ * slots ("ranges") are where the order matters, so *split is the smallest of
+ *   (a) the index of the first range that shares a slot with an earlier range of the call (judged on the full
+ *       extents: its stop would depend on how far the earlier one got),
+ *   (b) the index of the first range past FPX_MAX_RANGE_BATCH,
+ * and n.  Nothing at or past *split is applied: continue with in + *split (no refusal, nothing half applied).  A
+ * range re-proposed after a leader change is what makes two ranges of one batch overlap, so a split is rare.
+ * Statuses of the records before the split: FPX_ERR_SLOT_RANGE for 0 <= slot_start <= slot_end <= slot_capacity
+ * broken (the lowest such index in *err_index; the other records are applied).  FPX_ERR_UNSUPPORTED unless
+ * protocol == FPX_MENCIUS and shard_count == 1 (a sharded log keeps the _first / MIN / _fill path above).
+ * n <= max_batch.  fpx_chosen_watermark afterwards is the first hole.  The _dev form runs on the engine's stream and
+ * writes the split to d_split; its status is collected by fpx_sync. */
+int fpx_mencius_replica_inbound(fpx_engine* e, const fpx_mencius_chosen* in, int32_t n, int32_t* split,
+                                int64_t* err_index);
+int fpx_mencius_replica_inbound_dev(fpx_engine* e, const fpx_mencius_chosen* d_in, int32_t n, int32_t* d_split);
 
 /* ---- Wire codec: the reference's protobuf bytes <-> the records above ---------------
  * Every actor's inbound serializer is ProtoSerializer (S/ProtoSerializer.scala:3-11:
@@ -421,7 +445,9 @@ int fpx_wire_encode_phase2b(fpx_engine* e, const fpx_p2b* in, int32_t n, uint8_t
                             int32_t* offsets, int64_t* err_index);
 int fpx_wire_encode_phase2b_dev(fpx_engine* e, const fpx_p2b* d_in, int32_t n, uint8_t* d_out, int32_t out_capacity,
                                 int32_t* d_offsets);
-/* LeaderInbound{nack{round}}; in[i].leader selects the destination and is not on the wire. */
+/* LeaderInbound{nack{round}}; in[i].leader selects the destination and is not on the wire.  The member is
+ * nack = 6 (S/multipaxos/MultiPaxos.proto:525-539), with protocol FPX_MENCIUS nack = 7
+ * (S/mencius/Mencius.proto:322-337, where field 6 is leader_info_request_batcher). */
 int fpx_wire_encode_nack(fpx_engine* e, const fpx_nack* in, int32_t n, uint8_t* out, int32_t out_capacity,
                          int32_t* offsets, int64_t* err_index);
 /* ReplicaInbound{chosen{slot, command_batch_or_noop}}: the value bytes of value_id v are
@@ -492,6 +518,40 @@ int fpx_wire_encode_vm_skip(fpx_engine* e, const fpx_vm_skip_rec* in, int32_t n,
                             int32_t* offsets, int64_t* err_index);
 int fpx_wire_encode_vm_skip_dev(fpx_engine* e, const fpx_vm_skip_rec* d_in, int32_t n, uint8_t* d_out,
                                 int32_t out_capacity, int32_t* d_offsets);
+
+/* ---- Wire codec of Compartmentalized Mencius' noop ranges and replica (protocol FPX_MENCIUS; any other:
+ * FPX_ERR_UNSUPPORTED) ----
+ * S/mencius/Mencius.proto: Phase2bNoopRange :178-187, Chosen :189-195, ChosenNoopRange :197-203, ProxyLeaderInbound
+ * :339-350, ReplicaInbound :363-371 {chosen = 1, chosen_noop_range = 2}.  Parsing rules, buffers, offsets[n+1] and
+ * out_capacity as for the calls above.  The Mencius Chosen has MultiPaxos's shape: fpx_wire_encode_chosen writes it.
+ *
+ * Decode a batch of ReplicaInbound into the records fpx_mencius_replica_inbound applies, DENSE: row i answers
+ * message i.  kind[i] = the member's field number.
+ *   1 chosen             {slot, slot + 1, value_id_base + i, 0}; values[2i], values[2i+1] = {off, len} of
+ *                        command_batch_or_noop in bytes (located, not parsed; a second one is FPX_ERR_WIRE)
+ *   2 chosen_noop_range  {start, end, FPX_VALUE_NOOP, 0}
+ *   0 no member          {0, 0, FPX_VALUE_NOOP, 0}, a row that covers no slot.  The reference's replica stops with
+ *                        logger.fatal("Empty ReplicaInbound encountered."); that decision is the caller's, by kind.
+ * values of the rows of kinds 0 and 2 are {0, 0}; a message that fails (FPX_ERR_WIRE) gets kind 0 and that row. */
+int fpx_wire_decode_mencius_replica_inbound(fpx_engine* e, const uint8_t* bytes, const int32_t* offsets, int32_t n,
+                                            int32_t value_id_base, int32_t* kind, fpx_mencius_chosen* recs,
+                                            int32_t* values, int64_t* err_index);
+int fpx_wire_decode_mencius_replica_inbound_dev(fpx_engine* e, const uint8_t* d_bytes, const int32_t* d_offsets,
+                                                int32_t n, int32_t value_id_base, int32_t* d_kind,
+                                                fpx_mencius_chosen* d_recs, int32_t* d_values);
+/* The acceptor's replies of fpx_mencius_acceptor_noop_range: ProxyLeaderInbound{phase2b_noop_range = 5
+ * {acceptor_group_index = (dst >> 16) % num_acceptor_groups, acceptor_index = dst & 0xffff, start, end, round}}.
+ * Decoding it with FPX_WIRE_MENCIUS_PROXYLEADER_INBOUND gives back the record. */
+int fpx_wire_encode_mencius_phase2b_range(fpx_engine* e, const fpx_p2b_range* in, int32_t n, uint8_t* out,
+                                          int32_t out_capacity, int32_t* offsets, int64_t* err_index);
+int fpx_wire_encode_mencius_phase2b_range_dev(fpx_engine* e, const fpx_p2b_range* d_in, int32_t n, uint8_t* d_out,
+                                              int32_t out_capacity, int32_t* d_offsets);
+/* The proxy leader's ChosenNoopRange of fpx_mencius_range_phase2b, sent to every replica:
+ * ReplicaInbound{chosen_noop_range = 2 {start, end}}. */
+int fpx_wire_encode_mencius_chosen_range(fpx_engine* e, const fpx_chosen_range* in, int32_t n, uint8_t* out,
+                                         int32_t out_capacity, int32_t* offsets, int64_t* err_index);
+int fpx_wire_encode_mencius_chosen_range_dev(fpx_engine* e, const fpx_chosen_range* d_in, int32_t n, uint8_t* d_out,
+                                             int32_t out_capacity, int32_t* d_offsets);
 
 /* ---- EPaxos replica (S/epaxos/Replica.scala) ------------------------------
  * One fpx_epaxos handle = one replica's cmdLog (:298-330) and leaderStates
