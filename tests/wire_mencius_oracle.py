@@ -102,15 +102,23 @@ class Replica:
         self.lg, self.cap, self.retired = lg, capacity, 0
         self.log = np.full(capacity, -1, dtype=np.int32)
 
-    def split(self, recs):
-        recs = np.ascontiguousarray(recs, dtype=MENCIUS_CHOSEN)
-        return lib().fpo_mencius_split(recs.ctypes.data, len(recs), self.lg, self.cap)
+    def _bound(self, limit):
+        """The slot bound of a call: the engine's live bound (base + slot_capacity) of a log that slides, so that
+        one oracle log can cover a log many times the engine's capacity; the whole log by default."""
+        if limit is None:
+            return self.cap
+        assert 0 <= limit <= self.cap, (limit, self.cap)
+        return limit
 
-    def apply(self, recs):
-        """-> (status, err_index)"""
+    def split(self, recs, limit=None):
+        recs = np.ascontiguousarray(recs, dtype=MENCIUS_CHOSEN)
+        return lib().fpo_mencius_split(recs.ctypes.data, len(recs), self.lg, self._bound(limit))
+
+    def apply(self, recs, limit=None):
+        """-> (status, err_index).  A record past `limit` is FPX_ERR_SLOT_RANGE, as past the engine's live bound."""
         recs = np.ascontiguousarray(recs, dtype=MENCIUS_CHOSEN)
         err = C.c_int64(-1)
-        st = lib().fpo_mencius_apply(recs.ctypes.data, len(recs), self.lg, self.cap, self.retired,
+        st = lib().fpo_mencius_apply(recs.ctypes.data, len(recs), self.lg, self._bound(limit), self.retired,
                                      self.log.ctypes.data, C.byref(err))
         return st, err.value
 
