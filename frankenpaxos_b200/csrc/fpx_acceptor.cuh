@@ -174,7 +174,11 @@ __device__ __forceinline__ void acceptor_apply(const AcceptorParams& P, int4* ou
           // states(slot) = State(voteRound = round, voteValue) (:205-208)
           if (loc >= 0) {   // (a retired slot's vote is never read again: Phase1b starts at the chosen watermark, :171-179)
             cell[u] = ((unsigned long long)(uint32_t)(r + 1) << 32) | (uint32_t)rec[u].z;
+#ifdef FPX_PROFILE_ACC_RED   // attribution build only (profiles/README.md): wrong state, re-votes go undetected
+            red_max_u64(&P.votes[cell_index(g, loc, vix)], cell[u]);
+#else
             old[u] = atomicMax(&P.votes[cell_index(g, loc, vix)], cell[u]);
+#endif
           }
           // maxVotedSlot = max(maxVotedSlot, slot) (:209): thread-private column
           atomicMax(&s_mv[key * kAT + threadIdx.x], rec[u].x);

@@ -28,6 +28,7 @@ struct ArmParams {
   int32_t vanilla;
   RangeTable rng;      // mencius: one-slot Phase2aNoopRange keys share the key space (check_rng != 0)
   int32_t check_rng;
+  int32_t fast;        // certify the batch for plain row stores (not vanilla, not check_rng; DevStatus::fresh_rows)
 };
 
 __device__ __forceinline__ void note_arm_conflict(const ArmParams& P, int slot, int round) {
@@ -143,31 +144,47 @@ __device__ __forceinline__ void vm_retired_request(const ArmParams& P, const int
     report_error(P.st, FPX_ERR_BAD_ACCEPTOR, i);
 }
 
-constexpr int kArmUnroll = 8;
+constexpr int kArmUnroll = 8;            // records in flight per lane in the CAS loop
+constexpr int kArmUnrollCertified = 6;   // the same in the certifying kernel's fallback: 8 spills at the 64-register cap
 constexpr int kArmThreads = 1024;   // one CTA of 32 warps per SM, at most one wave (grid-stride loop)
+
+// 16-byte store tagged evict_last, the policy created in place (as in ld_u64_evict_last)
+__device__ __forceinline__ void st_v4_evict_last(uint32_t* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("{ .reg .b64 pol; createpolicy.fractional.L2::evict_last.b64 pol, 1.0; "
+               "st.global.L1::no_allocate.L2::cache_hint.v4.u32 [%0], {%1, %2, %3, %4}, pol; }"
+               ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+// The row an arm leaves in a never-touched row -- {round, value, no stamps} -- written whole: every 32-byte
+// sector is covered by the stores, so L2 takes the line without reading it from DRAM first.  Tagged
+// evict_last like the CAS path's header load: the tally's stamps and sweep come back to the row in the step.
+__device__ __forceinline__ void store_fresh_row(uint32_t* row, int row_words, int round, int value) {
+  st_v4_evict_last(row, (uint32_t)round, (uint32_t)value, kStampEmpty, kStampEmpty);
+  for (int w = 4; w < row_words; w += 4) st_v4_evict_last(row + w, kStampEmpty, kStampEmpty, kStampEmpty, kStampEmpty);
+}
 
 // The arm work of warp `gwarp` of `total_warps` (arm_kernel; also called from the acceptor kernel when
 // fpx_step_dev runs both roles in one launch).  Warp-strided 32-record chunks; per lane kArmUnroll
 // independent record loads, then kArmUnroll independent header CASes, are in flight before any result is
 // used.  Only the row index and the CAS result stay live across the round trip; the rare slow paths
 // (key exists, second round of a slot, vanilla self vote) re-read their record.
+template <int kUnroll>
 __device__ __forceinline__ int arm_chunks(const ArmParams& P, int gwarp, int total_warps, int lane) {
   const Geometry& g = P.g;
   const int n_chunks = (P.n + 31) >> 5;
   int max_local = -1;
-  for (int c0 = gwarp * kArmUnroll; c0 < n_chunks; c0 += total_warps * kArmUnroll) {
-    unsigned long long old[kArmUnroll];
-    unsigned long long want[kArmUnroll];
-    int local[kArmUnroll];          // row of the record, -1: not a valid arm, kLocalRetired: vanilla, retired slot
+  for (int c0 = gwarp * kUnroll; c0 < n_chunks; c0 += total_warps * kUnroll) {
+    unsigned long long old[kUnroll];
+    unsigned long long want[kUnroll];
+    int local[kUnroll];          // row of the record, -1: not a valid arm, kLocalRetired: vanilla, retired slot
     {
-      int4 rec[kArmUnroll];
+      int4 rec[kUnroll];
 #pragma unroll
-      for (int u = 0; u < kArmUnroll; ++u) {
+      for (int u = 0; u < kUnroll; ++u) {
         int i = (c0 + u) * 32 + lane;
         rec[u] = (c0 + u < n_chunks && i < P.n) ? ld_stream(P.in + i) : make_int4(-1, 0, 0, 0);  // {slot, round, value_id, dst}
       }
 #pragma unroll
-      for (int u = 0; u < kArmUnroll; ++u) {
+      for (int u = 0; u < kUnroll; ++u) {
         int i = (c0 + u) * 32 + lane;
         local[u] = -1;
         old[u] = 0;
@@ -194,17 +211,25 @@ __device__ __forceinline__ int arm_chunks(const ArmParams& P, int gwarp, int tot
             local[u] = l;
             want[u] = ((unsigned long long)(uint32_t)rec[u].z << 32) | (uint32_t)rec[u].y;
             const unsigned long long* hdr = (const unsigned long long*)(P.pl.rows + (size_t)l * g.row_words);
+#ifdef FPX_PROFILE_ARM_STORE   // attribution build only (profiles/README.md): no load, no CAS, wrong state
+            (void)hdr;
+            store_fresh_row(P.pl.rows + (size_t)l * g.row_words, g.row_words, rec[u].y, rec[u].z);
+            old[u] = kU64Empty;
+#else
             old[u] = P.vanilla ? __ldcg(hdr) : ld_u64_evict_last(hdr);
+#endif
           }
         }
       }
     }
 #pragma unroll
-    for (int u = 0; u < kArmUnroll; ++u)
+    for (int u = 0; u < kUnroll; ++u)
+#if !defined(FPX_PROFILE_ARM_NOCAS) && !defined(FPX_PROFILE_ARM_STORE)   // attribution builds: no CAS, wrong state
       if (local[u] >= 0 && old[u] == kU64Empty)
         old[u] = atomicCAS((unsigned long long*)(P.pl.rows + (size_t)local[u] * g.row_words), kU64Empty, want[u]);
+#endif
 #pragma unroll
-    for (int u = 0; u < kArmUnroll; ++u) {
+    for (int u = 0; u < kUnroll; ++u) {
       if (c0 + u >= n_chunks) break;
       int i = (c0 + u) * 32 + lane;
       bool won = local[u] >= 0 && old[u] == kU64Empty;       // Pending(phase2a, {}) created (:213)
@@ -270,10 +295,95 @@ __device__ __forceinline__ void arm_resolve_conflicts(const ArmParams& P) {
   if (threadIdx.x == 0) P.st->n_arm_conflicts = 0;
 }
 
-__global__ void __launch_bounds__(kArmThreads, 1) arm_kernel(ArmParams P) {
+// Fast-path pass 1 of warp `gwarp`: can the batch be armed by plain stores?  Every record must be valid (slot in
+// this shard's live window, round in range), slots strictly increasing over every adjacent pair of the batch --
+// so no key repeats and no slot is armed in a second round -- and every ordinal at or above fresh_rows, so every
+// row it arms still holds the creation value and the CAS would have won.  Sets *bad otherwise.  Returns the
+// largest ordinal of a record in the live window (the rows either path may write), or -1.
+constexpr int kArmCertUnroll = 4;
+__device__ __forceinline__ int arm_certify(const ArmParams& P, bool* bad) {
   const int lane = threadIdx.x & 31;
-  const int max_local = arm_chunks(P, blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), gridDim.x * (blockDim.x >> 5), lane);
-  if (lane == 0 && max_local >= 0) atomicMax(&P.st->max_armed_local, max_local);
+  const int gwarp = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), total_warps = gridDim.x * (blockDim.x >> 5);
+  const Geometry& g = P.g;
+  const int fresh = __ldcg(&P.st->fresh_rows);
+  const int n_chunks = (P.n + 31) >> 5;
+  int top = -1;
+  for (int c0 = gwarp * kArmCertUnroll; c0 < n_chunks; c0 += total_warps * kArmCertUnroll) {
+    int4 rec[kArmCertUnroll];
+    int nxt[kArmCertUnroll];   // lane 31: the slot of the record after the chunk
+#pragma unroll
+    for (int u = 0; u < kArmCertUnroll; ++u) {
+      const int i = (c0 + u) * 32 + lane;
+      rec[u] = i < P.n ? __ldcg(P.in + i) : make_int4(-1, 0, 0, 0);
+      nxt[u] = (lane == 31 && i + 1 < P.n) ? __ldcg(&P.in[i + 1].x) : 0;
+    }
+#pragma unroll
+    for (int u = 0; u < kArmCertUnroll; ++u) {
+      const int i = (c0 + u) * 32 + lane;
+      const int down = __shfl_down_sync(0xffffffffu, rec[u].x, 1);
+      if (i >= P.n) continue;
+      const int l = local_slot(g, rec[u].x);
+      if (l < 0) { *bad = true; continue; }
+      const int ord = g.base_local + ring_to_rel(g, l);
+      top = max(top, ord);
+      if ((uint32_t)rec[u].y > (uint32_t)FPX_MAX_ROUND || ord < fresh) *bad = true;
+      if (i + 1 < P.n && rec[u].x >= (lane == 31 ? nxt[u] : down)) *bad = true;
+    }
+  }
+  return top;
+}
+
+// Fast-path pass 2 of warp `gwarp` (a certified batch): every record creates its key (Pending(phase2a, {}),
+// ProxyLeader.scala:213), its row written whole by store_fresh_row, no load and no CAS.  The same chunks as
+// pass 1, whose loads left the records in L2.  win_bits stay unwritten: only arm_resolve_conflicts reads them,
+// and a batch without a repeated key notes no conflict.  Returns the largest ring index armed.
+__device__ __forceinline__ int arm_fresh(const ArmParams& P) {
+  const int lane = threadIdx.x & 31;
+  const int gwarp = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), total_warps = gridDim.x * (blockDim.x >> 5);
+  const Geometry& g = P.g;
+  const int n_chunks = (P.n + 31) >> 5;
+  int max_local = -1;
+  for (int c0 = gwarp * kArmCertUnroll; c0 < n_chunks; c0 += total_warps * kArmCertUnroll) {
+    int4 rec[kArmCertUnroll];
+#pragma unroll
+    for (int u = 0; u < kArmCertUnroll; ++u) {
+      const int i = (c0 + u) * 32 + lane;
+      rec[u] = i < P.n ? ld_stream(P.in + i) : make_int4(-1, 0, 0, 0);
+    }
+#pragma unroll
+    for (int u = 0; u < kArmCertUnroll; ++u) {
+      if ((c0 + u) * 32 + lane >= P.n) continue;
+      const int l = local_slot(g, rec[u].x);
+      store_fresh_row(P.pl.rows + (size_t)l * g.row_words, g.row_words, rec[u].y, rec[u].z);
+      max_local = max(max_local, l);
+    }
+  }
+  return __reduce_max_sync(0xffffffffu, max_local);
+}
+
+// One CTA of kArmThreads per SM; kCertify (P.fast): cooperative launch, one grid barrier between the passes.
+template <bool kCertify>
+__global__ void __launch_bounds__(kArmThreads, 1) arm_kernel(ArmParams P) {
+  __shared__ int s_top;
+  bool fast = false;
+  if (kCertify) {
+    if (threadIdx.x == 0) s_top = -1;
+    __syncthreads();
+    bool bad = false;
+    const int top = __reduce_max_sync(0xffffffffu, arm_certify(P, &bad));
+    if ((threadIdx.x & 31) == 0 && top >= 0) atomicMax(&s_top, top);
+    if (__syncthreads_or(bad) && threadIdx.x == 0) atomicOr(&P.st->arm_bad, 1u);
+    grid_sync(P.st);
+    fast = __ldcg(&P.st->arm_bad) == 0u;
+    // every CTA read fresh_rows before the barrier: the rows this batch writes leave the fresh region now
+    if (threadIdx.x == 0 && s_top >= 0) atomicMax(&P.st->fresh_rows, s_top + 1);
+    if (blockIdx.x == 0 && threadIdx.x == 0) P.st->arm_path = fast ? 2u : 1u;
+  }
+  const int max_local =
+      fast ? arm_fresh(P)
+           : arm_chunks<kCertify ? kArmUnrollCertified : kArmUnroll>(
+                 P, blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), gridDim.x * (blockDim.x >> 5), threadIdx.x & 31);
+  if ((threadIdx.x & 31) == 0 && max_local >= 0) atomicMax(&P.st->max_armed_local, max_local);
 
   // ---- last block: conflicting arms of one key
   __shared__ bool s_last;
@@ -285,7 +395,11 @@ __global__ void __launch_bounds__(kArmThreads, 1) arm_kernel(ArmParams P) {
   __syncthreads();
   if (!s_last) return;
   __threadfence();
-  if (threadIdx.x == 0) P.st->ticket = 0;
+  if (threadIdx.x == 0) {
+    P.st->ticket = 0;
+    P.st->arm_bad = 0;   // every CTA has read it (before its ticket)
+    if (!kCertify) P.st->arm_path = 1u;
+  }
   arm_resolve_conflicts(P);
 }
 

@@ -67,6 +67,13 @@ struct DevStatus {
                                         // into the table since (a moved slot's first key; its later keys share
                                         // the slot, so they leave with it)
   uint32_t rng_used;                    // mencius noop-range table: occupied entries
+  // Fresh frontier of the proxy-leader rows: every live-window ordinal u >= fresh_rows holds what fpx_create /
+  // recycle_kernel leave there (all 0xFF).  Raised to u + 1 by the arm and the tally, the writers of `rows` of
+  // the engines that take the arm's fast path; the window only slides past it (fpx_retire_below), fpx_reset
+  // puts it back to 0.  Vanilla Mencius and range-checking arms never take the fast path and leave it alone.
+  int32_t fresh_rows;
+  uint32_t arm_bad;                     // arm pass 1: the batch is not certified (reset by the launch's last CTA)
+  uint32_t arm_path;                    // path the LAST arm launch took: 1 per-record CAS, 2 certified plain stores
 };
 
 __device__ __forceinline__ unsigned long long global_timer_ns() {

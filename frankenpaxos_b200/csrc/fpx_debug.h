@@ -13,7 +13,7 @@ extern "C" {
 
 int fpx_debug_phase_times(fpx_engine* e, unsigned long long* acceptor8, unsigned long long* tally8);
 int fpx_debug_set_tally_path(fpx_engine* e, int32_t path);
-int fpx_debug_last_tally_path(fpx_engine* e);
+int fpx_debug_last_paths(fpx_engine* e, int32_t* out);
 int fpx_debug_set_acceptor_segments(fpx_engine* e, int32_t segments);
 int fpx_debug_set_tally_max_sub(fpx_engine* e, int32_t votes);
 int fpx_debug_set_counters(fpx_engine* e, uint32_t seq_base, uint32_t rseq_base, uint32_t rng_seq_base,

@@ -523,7 +523,7 @@ int fpx_debug_phase_times(fpx_engine* e, unsigned long long* acceptor8, unsigned
 }
 int64_t fpx_launch_count(const fpx_engine* e) { return e ? e->launches : 0; }
 // Undocumented test/profiling aids: force the tally's exact per-vote path (path = 2; 0 = automatic), and
-// which path the last tally launch took (1 sweep, 2 exact).
+// which paths the last tally and arm launches took.
 int fpx_debug_set_tally_path(fpx_engine* e, int32_t path) {
   if (!e || (path & ~6)) return FPX_ERR_INVALID_ARG;
   e->tally_path = path;
@@ -543,12 +543,14 @@ int fpx_debug_set_tally_max_sub(fpx_engine* e, int32_t votes) {
   e->tally_max_sub = votes == 0 ? kTallyMaxSub : votes;
   return FPX_OK;
 }
-int fpx_debug_last_tally_path(fpx_engine* e) {
-  if (!e) return FPX_ERR_INVALID_ARG;
-  uint32_t v = 0;
+// out[0]: the last tally launch's path (1 sweep, 2 exact); out[1]: the last arm launch's (1 per-record CAS,
+// 2 certified batch of fresh keys, plain row stores); 0 = no such launch since the engine was created or reset.
+int fpx_debug_last_paths(fpx_engine* e, int32_t* out) {
+  if (!e || !out) return FPX_ERR_INVALID_ARG;
   CK(e, cudaStreamSynchronize(e->stream));
-  CK(e, cudaMemcpy(&v, &e->st->ts_path, 4, cudaMemcpyDeviceToHost));
-  return (int)v;
+  CK(e, cudaMemcpy(&out[0], &e->st->ts_path, 4, cudaMemcpyDeviceToHost));
+  CK(e, cudaMemcpy(&out[1], &e->st->arm_path, 4, cudaMemcpyDeviceToHost));
+  return FPX_OK;
 }
 // Undocumented test aids: the host's 32-bit counters {seq_base (Phase2b stamps), rseq_base (Chosen log numbers),
 // rng_seq_base (Phase2bNoopRange stamps), vm_tag (vanilla Mencius batch tag)}, so that a test can start them just
@@ -590,6 +592,11 @@ static ArmParams arm_params(fpx_engine* e, const fpx_p2a* d_in, int32_t n, int v
   P.vanilla = vanilla;
   P.rng = RangeTable{e->rng_tab, (uint32_t)e->rng_cap - 1u, e->rng_cap};
   P.check_rng = e->unit_ranges;
+#if defined(FPX_PROFILE_ARM_NOCAS) || defined(FPX_PROFILE_ARM_STORE)
+  P.fast = 0;   // attribution builds time the per-record loop
+#else
+  P.fast = !vanilla && !P.check_rng;
+#endif
   return P;
 }
 
@@ -598,7 +605,11 @@ static int arm_launch(fpx_engine* e, const fpx_p2a* d_in, int32_t n, int vanilla
   if (c != FPX_OK || n == 0) return c;
   ArmParams P = arm_params(e, d_in, n, vanilla);
   int arm_blocks = std::min((n + kArmThreads * kArmUnroll - 1) / (kArmThreads * kArmUnroll), e->num_sms);
-  arm_kernel<<<arm_blocks, kArmThreads, 0, e->stream>>>(P);
+  void* args[] = {&P};
+  if (P.fast)
+    CK(e, cudaLaunchCooperativeKernel((const void*)arm_kernel<true>, dim3(arm_blocks), dim3(kArmThreads), args, 0, e->stream));
+  else
+    arm_kernel<false><<<arm_blocks, kArmThreads, 0, e->stream>>>(P);
   e->launches++;
   CK(e, cudaGetLastError());
   return FPX_OK;

@@ -651,6 +651,9 @@ __global__ void __launch_bounds__(kTT, 1024 / kTT) tally_kernel(TallyParams P) {
     if (blockIdx.x == 0 && tid == 0) {
       // every CTA is past its reads of the statistics (barrier after phase C): reset them for the next launch
       P.st->n_chosen = (int)(out_base + total);
+      // every row this launch wrote (blind stamps, exact path, sweep) lies in the window of its votes, and a
+      // stray vote's stamp makes an unarmed row stale as well
+      if (w_hi >= 0) P.st->fresh_rows = max(P.st->fresh_rows, g.base_local + w_hi + 1);
       P.st->ts_min_local = INT_MAX; P.st->ts_max_local = -1;
       P.st->ts_min_round = INT_MAX; P.st->ts_max_round = INT_MIN;
       P.st->ts_flags = 0;

@@ -200,10 +200,21 @@ class Engine(_Handle):
         self._check(self._L.fpx_debug_get_counters(self.h, out.ctypes.data))
         return dict(zip(self.COUNTERS, (int(x) for x in out)))
 
+    def _last_paths(self):
+        out = np.zeros(2, dtype=np.int32)
+        self._check(self._L.fpx_debug_last_paths(self.h, out.ctypes.data))
+        return out
+
     @property
     def last_tally_path(self):
         """'sweep' / 'exact': what the last proxyleader_phase2b launch did."""
-        return {1: "sweep", 2: "exact"}.get(self._L.fpx_debug_last_tally_path(self.h), "none")
+        return {1: "sweep", 2: "exact"}.get(int(self._last_paths()[0]), "none")
+
+    @property
+    def last_arm_path(self):
+        """'cas' / 'fresh': what the last proxyleader_arm launch did (one CAS per record, or a batch certified as
+        fresh keys in strict slot order, armed by plain row stores)."""
+        return {1: "cas", 2: "fresh"}.get(int(self._last_paths()[1]), "none")
 
     # -- host-pointer calls (numpy in / numpy out)
     def proxyleader_arm(self, p2a):

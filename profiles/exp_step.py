@@ -20,6 +20,8 @@ ap.add_argument("--variants", default="default,acc_first,exact,default,acc_first
 ap.add_argument("--out", default="")
 ap.add_argument("--old-lib", action="store_true", help="time the round-1 build (profiles/_r1/libfpx.so) instead")
 ap.add_argument("--lib", default="", help="time another build of libfpx.so (tuning variants under profiles/_var/)")
+ap.add_argument("--wrong-state", action="store_true",
+                help="the build is an attribution variant (-DFPX_PROFILE_*, profiles/README.md): skip the result check")
 args = ap.parse_args()
 if args.old_lib:
     os.environ["FPX_LIB_OVERRIDE"] = os.path.join(ROOT, "profiles", "_r1", "libfpx.so")
@@ -105,7 +107,7 @@ for variant in args.variants.split(","):
             evs[s][j + 1].record(ext)
     t_host = (time.perf_counter() - t_host0) / S * 1e6
     r = eng.sync()
-    if "nored" not in variant:
+    if "nored" not in variant and not args.wrong_state:
         assert r.status == 0 and r.n_chosen == n and r.watermark == S * n, (r.status, r.n_chosen, r.watermark)
     step = evs[3][0].elapsed_time(evs[S - 1][5]) * 1e3 / (S - 3)
     per = {} if noev else {which: float(np.mean([evs[s][j].elapsed_time(evs[s][j + 1]) for s in range(3, S)])) * 1e3
@@ -121,7 +123,8 @@ for variant in args.variants.split(","):
     tt = np.array(tt[:8], dtype=np.int64)
     ta = np.array(ta[:6], dtype=np.int64)
     res = {"step_us": step, "host_enqueue_us_per_step": t_host, "kernels_us": per, "sum_kernels_us": sum(per.values()),
-           "tally_path": "r1" if args.old_lib else eng.last_tally_path,
+           "tally_path": eng.last_tally_path if hasattr(L, "fpx_debug_last_paths") else "n/a",
+           "arm_path": eng.last_arm_path if hasattr(L, "fpx_debug_last_paths") else "n/a",
            "tally_phases_us(A,bar,B,bar,C,bar,D)": (np.diff(tt) / 1e3).round(1).tolist(),
            "acceptor_phases_us(p1,bar,carry,p2,bar)": (np.diff(ta) / 1e3).round(1).tolist()}
     print(variant, json.dumps(res), flush=True)
