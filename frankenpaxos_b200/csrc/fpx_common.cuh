@@ -221,9 +221,12 @@ __device__ __forceinline__ unsigned lanemask_lt() {
   return m;
 }
 
+// err_word: min over errors of (index << 8 | -code), DevStatus's and ReadsDev's alike
+__device__ __forceinline__ void report_error(unsigned long long* err_word, int code, long long index) {
+  atomicMin(err_word, ((unsigned long long)index << 8) | (unsigned long long)(unsigned)(-code));
+}
 __device__ __forceinline__ void report_error(DevStatus* st, int code, long long index) {
-  unsigned long long w = ((unsigned long long)index << 8) | (unsigned long long)(unsigned)(-code);
-  atomicMin(&st->err_word, w);
+  report_error(&st->err_word, code, index);
 }
 
 // State is a RING of local_slots rows over the shard's residue class: ordinal u = slot / shard_count lives at

@@ -43,6 +43,16 @@ constexpr int kStepRing = 1024;
 // dynamic shared memory; a larger call is cut into several launches (tally_launch)
 constexpr int32_t kTallyMaxSub = (40 * 1024 / 4) * kChunkVotes;
 
+// The wire codec's device buffers of a handle (fpx_engine, fpx_epaxos), grown on demand: the host forms' copies of
+// their inputs and outputs, and the encoders' tile sums
+struct WireBuf { void* p = nullptr; size_t cap = 0; };
+struct WireStage {
+  WireBuf bytes, offs;                 // a message batch: bytes and offsets
+  WireBuf kind, rec, sender, out, arena, voffs, tiles;
+  WireBuf aux;                         // EPaxos: the encoder's output rows, the pack's local deps
+  WireBuf rw_scratch, rw_out;          // the replica decode's per-message and per-tile scratch, its host-form output
+};
+
 struct fpx_engine {
   CudaResources res;                   // every buffer, stream and event below
   fpx_config cfg;
@@ -70,10 +80,7 @@ struct fpx_engine {
   int32_t* mix = nullptr;                  // mencius: scratch of the mixed replica call (fpx_mencius_replica_inbound)
   // fpx_step_dev: CUDA events around the acceptor and tally kernels of the last kStepRing steps
   std::vector<cudaEvent_t> step_ev;        // [kStepRing][4], created on first use
-  // wire codec staging (grown on demand)
-  struct WireBuf { void* p = nullptr; size_t cap = 0; };
-  WireBuf w_bytes, w_offs, w_kind, w_rec, w_sender, w_out, w_tiles, w_arena, w_voffs;
-  WireBuf w_rw_scratch, w_rw_out;      // the replica decode's per-message and per-tile scratch, its host-form output
+  WireStage wire;
   DevStatus* st = nullptr;
   // multi-GPU exchange
   DevExchange* xch = nullptr;          // device copy of the exchange descriptor

@@ -143,7 +143,7 @@ __device__ __forceinline__ int wire_member_count(int inbound) { return inbound =
 // *sender: the server field of a vanilla Mencius Phase2a, Phase2b or Skip (their field 1), else -1.
 // kIn == kWireInVm: inbound 4 (the only one with a bool, a sender or a ClientRequest span: the other inbounds compile
 // without them); kWireInMenciusReplica: inbound 5, {slot, 0, value_off, value_len} or {start, end, 0, 0}.
-template <bool kShared, int kIn>
+template <int kIn, bool kShared>
 __device__ __forceinline__ bool wire_decode_one(int inbound, int lgroups, int agroups, WireReader<kShared> r, int* kind,
                                                 int4* out, bool* value_pos, int* sender) {
   constexpr bool kVm = kIn == kWireInVm, kMr = kIn == kWireInMenciusReplica;
@@ -282,6 +282,19 @@ __device__ __forceinline__ WireSpan wire_stage_span(const uint8_t* bytes, const 
   __syncthreads();
   return w;
 }
+// Message [a, b) of the span: false when it lies outside (offsets must be monotone), else f(reader, rebase) once, on
+// the staged window with rebase = w.base (window -> buffer offsets) or on global memory with rebase = 0.
+template <class F>
+__device__ __forceinline__ bool wire_read(const WireSpan& w, const uint8_t* s_buf, const uint8_t* bytes, long long a,
+                                          long long b, F&& f) {
+  if (!(w.sane && a <= b && a >= w.lo && b <= w.hi)) return false;
+  if (w.staged)
+    f(WireReader<true>{(uint32_t)__cvta_generic_to_shared(s_buf), nullptr, (uint32_t)(a - w.base), (uint32_t)(b - w.base), true},
+      (uint32_t)w.base);
+  else
+    f(WireReader<false>{0u, bytes, (uint32_t)a, (uint32_t)b, true}, 0u);
+  return true;
+}
 
 // kIn: kWireInPath (inbounds 0-3), kWireInVm (the vanilla Mencius inbound 4: the other instantiations compile without
 // its bool, sender and ClientRequest span) or kWireInMenciusReplica (inbound 5: dense fpx_mencius_chosen rows)
@@ -293,25 +306,16 @@ __global__ void __launch_bounds__(kWireDecThreads) wire_decode_kernel(WireDecode
   const int m0 = blockIdx.x * kWireDecThreads;
   const int m1 = min(P.n, m0 + kWireDecThreads);
   const WireSpan w = wire_stage_span(P.bytes, P.offs, P.n, m0, m1, s_buf);
-  const long long lo = w.lo, hi = w.hi, base = w.base;
-  const bool sane = w.sane, staged = w.staged;
   const int i = m0 + threadIdx.x;
   if (i >= m1) return;
-  const long long a = P.offs[i], b = P.offs[i + 1];
   int kind = 0, sender = -1;
   int4 rec = make_int4(0, 0, 0, 0);
-  bool ok = sane && a <= b && a >= lo && b <= hi;      // offsets must be monotone
-  if (ok) {
+  bool ok = false;
+  wire_read(w, s_buf, P.bytes, P.offs[i], P.offs[i + 1], [&](auto r, uint32_t rebase) {
     bool value_pos = false;
-    if (staged) {
-      WireReader<true> r{(uint32_t)__cvta_generic_to_shared(s_buf), nullptr, (uint32_t)(a - base), (uint32_t)(b - base), true};
-      ok = wire_decode_one<true, kIn>(inbound, P.lgroups, P.agroups, r, &kind, &rec, &value_pos, &sender);
-      if (ok && value_pos) rec.z += (int)base;                  // window -> buffer offsets
-    } else {
-      WireReader<false> r{0u, P.bytes, (uint32_t)a, (uint32_t)b, true};
-      ok = wire_decode_one<false, kIn>(inbound, P.lgroups, P.agroups, r, &kind, &rec, &value_pos, &sender);
-    }
-  }
+    ok = wire_decode_one<kIn>(inbound, P.lgroups, P.agroups, r, &kind, &rec, &value_pos, &sender);
+    if (ok && value_pos) rec.z += (int)rebase;
+  });
   if (!ok) report_error(P.st, FPX_ERR_WIRE, i);
   if (kMr) {
     // Chosen(slot, v) -> {slot, slot + 1, value_id_base + i}, ChosenNoopRange(s, e) -> {s, e, Noop}; no member (or a
@@ -622,21 +626,14 @@ __global__ void __launch_bounds__(kWireDecThreads) ep_wire_decode_kernel(EpWireD
   const WireSpan w = wire_stage_span(P.bytes, P.offs, P.n, m0, m1, s_buf);
   const int i = m0 + threadIdx.x;
   if (i >= m1) return;
-  const long long a = P.offs[i], b = P.offs[i + 1];
   const int n = P.replicas;
   int32_t* row = P.rows + (long long)i * (EW_DEPS + n);
   EpWireMsg m = ep_wire_fresh();
   int kind = 0, code = FPX_ERR_WIRE;
-  if (w.sane && a <= b && a >= w.lo && b <= w.hi) {      // offsets must be monotone
-    if (w.staged) {
-      WireReader<true> r{(uint32_t)__cvta_generic_to_shared(s_buf), nullptr, (uint32_t)(a - w.base), (uint32_t)(b - w.base), true};
-      code = ep_wire_decode_one(r, n, &kind, m, row + EW_DEPS);
-      m.voff += (uint32_t)w.base;                         // window -> buffer offsets
-    } else {
-      WireReader<false> r{0u, P.bytes, (uint32_t)a, (uint32_t)b, true};
-      code = ep_wire_decode_one(r, n, &kind, m, row + EW_DEPS);
-    }
-  }
+  wire_read(w, s_buf, P.bytes, P.offs[i], P.offs[i + 1], [&](auto r, uint32_t rebase) {
+    code = ep_wire_decode_one(r, n, &kind, m, row + EW_DEPS);
+    m.voff += rebase;
+  });
   if (code != FPX_OK) {
     report_error(P.st, code, i);
     *(volatile uint32_t*)P.refused = P.tag;
@@ -771,24 +768,29 @@ __host__ __device__ constexpr int wire_small_max(int kind) {
   return kind == kWireNack || kind == kWireMenciusNack ? kWireMaxNack : kind == kWireMenciusP2bRange ? kWireMaxP2bRange
        : kind == kWireMenciusChosenRange ? kWireMaxChosenRange : kWireMaxP2b;
 }
-// encoders whose messages carry a value from the arena: size -> scan -> wire_emit_valued_kernel
+// encoders whose messages carry a value from the arena: size -> scan -> wire_gather_emit_kernel
 __host__ __device__ constexpr bool wire_gathers(int kind) {
   return kind == kWireChosen || kind == kWireVmReply || kind == kWireVmChosen || kind == kWireVmPhase2a;
 }
 
-struct WireEncodeParams {
-  const void* in;             // fpx_p2b (int4) | fpx_nack (int2) | fpx_chosen (int2) | fpx_p2a | fpx_vm_skip_rec
+// What every encoder's params hold (as their member `enc`): n records in, n messages out.
+struct WireEnc {
   int32_t n;
   uint8_t* out;               // 16-byte aligned
   int32_t out_capacity;
   int32_t* offs;              // n + 1
   uint32_t* tile_sum;         // [tiles] bytes per tile, then (after the scan) [tiles + 1] exclusive offsets
-  // value-gathering encoders: the value bytes of value_id v are arena[value_offs[v] .. value_offs[v + 1])
-  const uint8_t* arena;
+  const uint8_t* src;         // the gathered bytes: the value arena, or the request batch
+  unsigned long long* err_word;
+};
+
+struct WireEncodeParams {
+  WireEnc enc;
+  const void* in;             // fpx_p2b (int4) | fpx_nack (int2) | fpx_chosen (int2) | fpx_p2a | fpx_vm_skip_rec
+  // value-gathering encoders: the value bytes of value_id v are enc.src[value_offs[v] .. value_offs[v + 1])
   const int32_t* value_offs;
   int32_t num_values;
   int32_t servers;            // kWireVmPhase2a: sending_server = slot mod servers
-  DevStatus* st;
   int32_t agroups;            // kWireMenciusP2bRange: acceptor_group_index = (dst >> 16) mod agroups
 };
 
@@ -862,7 +864,7 @@ __device__ __forceinline__ int wire_msg_size(const WireMsg& m) {
 }
 
 template <int KIND>
-__device__ __forceinline__ int wire_size_of(const WireEncodeParams& P, int i, bool* bad) {
+__device__ __forceinline__ int wire_size_of(const WireEncodeParams& P, int i, int* code) {
   if (KIND == kWirePhase2b) {
     int4 r = ((const int4*)P.in)[i];
     // ProxyLeaderInbound{phase2b = 2}: 0x12, len (< 128: one byte), four int32 fields
@@ -890,34 +892,119 @@ __device__ __forceinline__ int wire_size_of(const WireEncodeParams& P, int i, bo
     int2 r = ((const int2*)P.in)[i];
     return 2 + 2 + wire_int32_size(r.x) + wire_int32_size(r.y);   // ReplicaInbound{chosen_noop_range = 2 {start, end}}
   } else {
-    const WireMsg m = wire_msg<KIND>(P, i, bad);
-    return *bad ? 0 : wire_msg_size(m);
+    bool bad = false;
+    const WireMsg m = wire_msg<KIND>(P, i, &bad);
+    if (bad) *code = FPX_ERR_INVALID_ARG;
+    return bad ? 0 : wire_msg_size(m);
   }
 }
 
-// pass 1: bytes per tile of kWireEncTile replies
+// An encoder is a codec C: wire_size_kernel<C> and wire_gather_emit_kernel<C> take its C::Params, which hold a WireEnc
+// as `enc`, and ask it for
+//   size_of(P, i, &code)          record i's message bytes; 0 when it sets *code (the record is bad)
+//   msg(P, i, &code), size(P, m)  a gathering encoder's message descriptor of record i and its bytes
+//   head(P, m, p, &gsrc, &glen)   writes message m at p but for the glen bytes gathered from enc.src + gsrc, and
+//                                 returns where those go
+//   stand_down(P)                 the call encodes nothing at all
+// WireKindCodec<KIND>: the WireEncodeParams encoders; only the wire_gathers kinds are emitted through msg / head.
 template <int KIND>
-__global__ void __launch_bounds__(kWireEncThreads) wire_size_kernel(WireEncodeParams P) {
+struct WireKindCodec {
+  using Params = WireEncodeParams;
+  using Msg = WireMsg;
+  static __device__ __forceinline__ bool stand_down(const Params&) { return false; }
+  static __device__ __forceinline__ int size_of(const Params& P, int i, int* code) { return wire_size_of<KIND>(P, i, code); }
+  static __device__ __forceinline__ Msg msg(const Params& P, int i, int* code) {
+    bool bad = false;
+    const WireMsg m = wire_msg<KIND>(P, i, &bad);
+    if (bad) *code = FPX_ERR_INVALID_ARG;
+    return m;
+  }
+  static __device__ __forceinline__ int size(const Params&, const Msg& m) { return wire_msg_size(m); }
+  // the head, a Noop and the trailing isRevocation; the arena's value bytes go between the last two
+  static __device__ __forceinline__ uint8_t* head(const Params&, const Msg& m, uint8_t* p, int* gsrc, int* glen) {
+    *p++ = (uint8_t)m.outer; p = wire_put_varint(p, (unsigned long long)wire_msg_body(m));
+    if (m.nf > 0) p = wire_put_int32(p, 1, m.f0);
+    if (m.nf > 1) p = wire_put_int32(p, 2, m.f1);
+    if (m.nf > 2) p = wire_put_int32(p, 3, m.f2);
+    int vlen = 0;
+    if (m.vfield) {
+      *p++ = (uint8_t)(m.vfield << 3 | 2); p = wire_put_varint(p, (unsigned long long)m.vlen);
+      if (m.noop) { *p++ = 0x12; *p++ = 0x00; }                // CommandOrNoop{noop = 2 {}}
+      else vlen = m.vlen;
+    }
+    if (m.revocation) { p[vlen] = 0x18; p[vlen + 1] = 0x00; }   // Chosen.isRevocation = 3: false
+    *gsrc = m.src; *glen = vlen;
+    return p;
+  }
+};
+
+// pass 1 of every encoder: bytes per tile of kWireEncTile records.  A thread reports its lowest bad record: the
+// error word keeps the lowest index of all.
+template <class C>
+__global__ void __launch_bounds__(kWireEncThreads) wire_size_kernel(typename C::Params P) {
+  if (C::stand_down(P)) return;
   __shared__ uint32_t s_w[kWireEncThreads / 32];
   uint32_t sum = 0;
-  bool bad = false;
-  int first_bad = INT_MAX;
   for (int u = 0; u < kWireEncPer; ++u) {
-    int i = blockIdx.x * kWireEncTile + (int)threadIdx.x * kWireEncPer + u;
-    if (i < P.n) {
-      bool b = false;
-      sum += (uint32_t)wire_size_of<KIND>(P, i, &b);
-      if (b) { bad = true; first_bad = min(first_bad, i); }
+    const int i = blockIdx.x * kWireEncTile + (int)threadIdx.x * kWireEncPer + u;
+    if (i < P.enc.n) {
+      int code = FPX_OK;
+      sum += (uint32_t)C::size_of(P, i, &code);
+      if (code != FPX_OK) report_error(P.enc.err_word, code, i);
     }
   }
-  if (bad) report_error(P.st, FPX_ERR_INVALID_ARG, first_bad);
   sum = __reduce_add_sync(0xffffffffu, sum);
   if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = sum;
   __syncthreads();
   if (threadIdx.x == 0) {
     uint32_t t = 0;
     for (int w = 0; w < kWireEncThreads / 32; ++w) t += s_w[w];
-    P.tile_sum[blockIdx.x] = t;
+    P.enc.tile_sum[blockIdx.x] = t;
+  }
+}
+
+// pass 3 of the gathering encoders (after tile_offsets_kernel): a message's head by its record's thread, its gathered
+// bytes by the warps of the CTA (lane-strided copy)
+template <class C>
+__global__ void __launch_bounds__(kWireEncThreads) wire_gather_emit_kernel(typename C::Params P) {
+  if (C::stand_down(P)) return;
+  __shared__ uint32_t s_dst[kWireEncTile];     // where each message's gathered bytes go
+  __shared__ int32_t s_src[kWireEncTile], s_len[kWireEncTile];
+  const uint32_t tiles = gridDim.x;
+  if (__ldcg(&P.enc.tile_sum[tiles]) > (uint32_t)P.enc.out_capacity) {   // output buffer too small
+    if (blockIdx.x == 0 && threadIdx.x == 0) report_error(P.enc.err_word, FPX_ERR_INVALID_ARG, 0);
+    return;
+  }
+  const uint32_t gbase = __ldcg(&P.enc.tile_sum[blockIdx.x]);
+  uint32_t run = 0;
+  for (int u = 0; u < kWireEncPer; ++u) {
+    const int i = blockIdx.x * kWireEncTile + u * kWireEncThreads + threadIdx.x;
+    const int slotix = u * kWireEncThreads + threadIdx.x;
+    int code = FPX_OK;
+    typename C::Msg m{};
+    if (i < P.enc.n) m = C::msg(P, i, &code);
+    const uint32_t sz = i < P.enc.n && code == FPX_OK ? (uint32_t)C::size(P, m) : 0u;
+    uint32_t tot;
+    const uint32_t off = run + cta_scan<kWireEncThreads, true>(sz, ScanSum(), &tot);
+    run += tot;
+    s_len[slotix] = 0;
+    if (i < P.enc.n) P.enc.offs[i] = (int32_t)(gbase + off);
+    if (sz) {
+      int gsrc = 0, glen = 0;
+      const uint8_t* gdst = C::head(P, m, P.enc.out + gbase + off, &gsrc, &glen);
+      s_dst[slotix] = (uint32_t)(gdst - P.enc.out);
+      s_src[slotix] = gsrc;
+      s_len[slotix] = glen;
+    }
+  }
+  if (blockIdx.x == tiles - 1 && threadIdx.x == 0) P.enc.offs[P.enc.n] = (int32_t)(gbase + run);
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int k = warp; k < kWireEncTile; k += kWireEncThreads / 32) {
+    const int len = s_len[k];
+    const uint8_t* src = P.enc.src + s_src[k];
+    uint8_t* dst = P.enc.out + s_dst[k];
+    for (int j = lane; j < len; j += 32) dst[j] = __ldg(src + j);
   }
 }
 
@@ -940,7 +1027,7 @@ __global__ void __launch_bounds__(kWireEncThreads) wire_emit_small_kernel(WireEn
     const int i = i0 + u;
     sz[u] = 0;
     rec[u] = make_int4(0, 0, 0, 0);
-    if (i < P.n) {
+    if (i < P.enc.n) {
       if (KIND == kWirePhase2b) {
         rec[u] = __ldcg((const int4*)P.in + i);      // second read of the records: L2
         sz[u] = 2 + 4 + wire_int32_size(rec[u].x) + wire_int32_size(rec[u].y) + wire_int32_size(rec[u].z) +
@@ -971,21 +1058,21 @@ __global__ void __launch_bounds__(kWireEncThreads) wire_emit_small_kernel(WireEn
   }
   // bytes of all tiles before this one (and, for the last tile, the grand total)
   unsigned long long gb = 0;
-  for (int t = threadIdx.x; t < tile; t += kWireEncThreads) gb += __ldcg(&P.tile_sum[t]);
+  for (int t = threadIdx.x; t < tile; t += kWireEncThreads) gb += __ldcg(&P.enc.tile_sum[t]);
   gb = cta_reduce<kWireEncThreads>(gb, ScanSum());
   uint32_t run;
   uint32_t off = cta_scan<kWireEncThreads, true>(mine, ScanSum(), &run);
-  const bool fits = gb + run <= (unsigned long long)P.out_capacity;
-  if (!fits && gb <= (unsigned long long)P.out_capacity && threadIdx.x == 0)
-    report_error(P.st, FPX_ERR_INVALID_ARG, 0);      // output buffer too small
+  const bool fits = gb + run <= (unsigned long long)P.enc.out_capacity;
+  if (!fits && gb <= (unsigned long long)P.enc.out_capacity && threadIdx.x == 0)
+    report_error(P.enc.err_word, FPX_ERR_INVALID_ARG, 0);      // output buffer too small
   const uint32_t gbase = (uint32_t)gb;
   const uint32_t phase = gbase & 15u;
   uint8_t* p = s_out + phase + off;
 #pragma unroll
   for (int u = 0; u < kWireEncPer; ++u) {
     const int i = i0 + u;
-    if (i >= P.n) break;
-    P.offs[i] = (int32_t)(gbase + off);
+    if (i >= P.enc.n) break;
+    P.enc.offs[i] = (int32_t)(gbase + off);
     off += sz[u];
     if (KIND == kWirePhase2b) {
       *p++ = 0x12; *p++ = (uint8_t)(sz[u] - 2);
@@ -1012,13 +1099,13 @@ __global__ void __launch_bounds__(kWireEncThreads) wire_emit_small_kernel(WireEn
       p = wire_put_int32(p, 1, rec[u].y);
     }
   }
-  if (tile == tiles - 1 && threadIdx.x == 0) P.offs[P.n] = (int32_t)(gbase + run);
+  if (tile == tiles - 1 && threadIdx.x == 0) P.enc.offs[P.enc.n] = (int32_t)(gbase + run);
   __syncthreads();
   if (!fits) return;
   // global [gbase, gbase + run) <- shared [phase, phase + run): aligned 16-byte chunks in the middle
   const uint32_t end = phase + run;
   const uint32_t body_lo = phase ? 16u : 0u, body_hi = end & ~15u;
-  uint8_t* g0 = P.out + (gbase - phase);     // 16-byte aligned
+  uint8_t* g0 = P.enc.out + (gbase - phase);     // 16-byte aligned
   if (body_hi > body_lo) {
     for (uint32_t k = body_lo + threadIdx.x * 16u; k < body_hi; k += kWireEncThreads * 16u)
       *(uint4*)(g0 + k) = *(const uint4*)(s_out + k);
@@ -1027,82 +1114,21 @@ __global__ void __launch_bounds__(kWireEncThreads) wire_emit_small_kernel(WireEn
   for (uint32_t k = max(body_hi, max(body_lo, phase)) + threadIdx.x; k < end; k += kWireEncThreads) g0[k] = s_out[k];
 }
 
-// pass 3 of the value-gathering encoders (wire_gathers): a message's head (and a Noop, and the trailing
-// isRevocation) by its thread, its value bytes by the warps of the CTA (lane-strided copy)
-template <int KIND>
-__global__ void __launch_bounds__(kWireEncThreads) wire_emit_valued_kernel(WireEncodeParams P) {
-  __shared__ uint32_t s_dst[kWireEncTile];     // where each message's value bytes go
-  __shared__ int32_t s_src[kWireEncTile], s_len[kWireEncTile];
-  const uint32_t tiles = gridDim.x;
-  if (__ldcg(&P.tile_sum[tiles]) > (uint32_t)P.out_capacity) {   // output buffer too small
-    if (blockIdx.x == 0 && threadIdx.x == 0) report_error(P.st, FPX_ERR_INVALID_ARG, 0);
-    return;
-  }
-  const uint32_t gbase = __ldcg(&P.tile_sum[blockIdx.x]);
-  uint32_t run = 0;
-  for (int u = 0; u < kWireEncPer; ++u) {
-    const int i = blockIdx.x * kWireEncTile + u * kWireEncThreads + threadIdx.x;
-    const int slotix = u * kWireEncThreads + threadIdx.x;
-    bool bad = false;
-    WireMsg m{};
-    if (i < P.n) m = wire_msg<KIND>(P, i, &bad);
-    const uint32_t sz = i < P.n && !bad ? (uint32_t)wire_msg_size(m) : 0u;
-    uint32_t tot;
-    const uint32_t off = run + cta_scan<kWireEncThreads, true>(sz, ScanSum(), &tot);
-    run += tot;
-    s_len[slotix] = 0;
-    if (i < P.n) P.offs[i] = (int32_t)(gbase + off);
-    if (i < P.n && sz) {
-      uint8_t* p = P.out + gbase + off;
-      *p++ = (uint8_t)m.outer; p = wire_put_varint(p, (unsigned long long)wire_msg_body(m));
-      if (m.nf > 0) p = wire_put_int32(p, 1, m.f0);
-      if (m.nf > 1) p = wire_put_int32(p, 2, m.f1);
-      if (m.nf > 2) p = wire_put_int32(p, 3, m.f2);
-      int vlen = 0;
-      if (m.vfield) {
-        *p++ = (uint8_t)(m.vfield << 3 | 2); p = wire_put_varint(p, (unsigned long long)m.vlen);
-        if (m.noop) { *p++ = 0x12; *p++ = 0x00; }                // CommandOrNoop{noop = 2 {}}
-        else vlen = m.vlen;
-      }
-      if (m.revocation) { p[vlen] = 0x18; p[vlen + 1] = 0x00; }   // Chosen.isRevocation = 3: false
-      s_dst[slotix] = (uint32_t)(p - P.out);
-      s_src[slotix] = m.src;
-      s_len[slotix] = vlen;
-    }
-  }
-  if (blockIdx.x == tiles - 1 && threadIdx.x == 0) P.offs[P.n] = (int32_t)(gbase + run);
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int m = warp; m < kWireEncTile; m += kWireEncThreads / 32) {
-    const int len = s_len[m];
-    const uint8_t* src = P.arena + s_src[m];
-    uint8_t* dst = P.out + s_dst[m];
-    for (int k = lane; k < len; k += 32) dst[k] = __ldg(src + k);
-  }
-}
-
-
 // ---------------------------------------------------------------------------
 // EPaxos encoder: one canonical ReplicaInbound per record of a handler call's input and output rows (include/fpx.h
-// fpx_epaxos_wire_encode).  The size -> tile-sum -> emit passes of the gathering encoder above, with a message
-// descriptor of its own: the member's fields in number order by ep_wire_roles, the nested Instance / Ballot /
-// InstancePrefixSetProto written inline, the CommandOrNoop's bytes gathered from the arena by the CTA's warps.
+// fpx_epaxos_wire_encode).  The gathering encoder above with a codec of its own (EpWireCodec): the member's fields in
+// number order by ep_wire_roles, the nested Instance / Ballot / InstancePrefixSetProto written inline, the
+// CommandOrNoop's bytes gathered from the arena by the CTA's warps.
 // ---------------------------------------------------------------------------
 struct EpWireEncodeParams {
+  WireEnc enc;                // enc.src: the arena
   int32_t call, replicas, self, per_replica;
   const int32_t* in;          // [n][w_in]   the call's input rows
   const int32_t* rows;        // [n][w_out]  its replies / events / ballots
   int32_t w_in, w_out;
   const int32_t* cmd;         // the handle's cmdLog: value_id of the value-less Commit / Accept records
-  int32_t n;
-  uint8_t* out;
-  int32_t out_capacity;
-  int32_t* offs;              // n + 1
-  uint32_t* tile_sum;
-  const uint8_t* arena;
   const int32_t* value_offs;
   int32_t num_values;
-  DevStatus* st;
   const uint32_t* refused;    // a refused handler call leaves rows unspecified: nothing is encoded behind it
 };
 struct EpMsg {
@@ -1223,78 +1249,27 @@ __device__ __forceinline__ int ep_msg_size(const EpMsg& m, int n) {
   return 1 + wire_varint_size((unsigned long long)b) + b;
 }
 
-// pass 1: bytes per tile of kWireEncTile records
-__global__ void __launch_bounds__(kWireEncThreads) ep_wire_size_kernel(EpWireEncodeParams P) {
-  if (__ldcg(P.refused) != 0) return;
-  __shared__ uint32_t s_w[kWireEncThreads / 32];
-  uint32_t sum = 0;
-  int first_bad = INT_MAX;
-  for (int u = 0; u < kWireEncPer; ++u) {
-    const int i = blockIdx.x * kWireEncTile + (int)threadIdx.x * kWireEncPer + u;
-    if (i < P.n) {
-      bool b = false;
-      const EpMsg m = ep_enc_msg(P, i, &b);
-      sum += (uint32_t)ep_msg_size(m, P.replicas);
-      if (b) first_bad = min(first_bad, i);
-    }
-  }
-  if (first_bad != INT_MAX) report_error(P.st, FPX_ERR_INVALID_ARG, first_bad);
-  sum = __reduce_add_sync(0xffffffffu, sum);
-  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = sum;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t t = 0;
-    for (int w = 0; w < kWireEncThreads / 32; ++w) t += s_w[w];
-    P.tile_sum[blockIdx.x] = t;
-  }
-}
-
-// pass 3 (after tile_offsets_kernel): heads by the record's thread, value bytes by the CTA's warps
-__global__ void __launch_bounds__(kWireEncThreads) ep_wire_emit_kernel(EpWireEncodeParams P) {
-  if (__ldcg(P.refused) != 0) return;
-  __shared__ uint32_t s_dst[kWireEncTile];
-  __shared__ int32_t s_src[kWireEncTile], s_len[kWireEncTile];
-  const uint32_t tiles = gridDim.x;
-  if (__ldcg(&P.tile_sum[tiles]) > (uint32_t)P.out_capacity) {   // output buffer too small
-    if (blockIdx.x == 0 && threadIdx.x == 0) report_error(P.st, FPX_ERR_INVALID_ARG, 0);
-    return;
-  }
-  const uint32_t gbase = __ldcg(&P.tile_sum[blockIdx.x]);
-  uint32_t run = 0;
-  for (int u = 0; u < kWireEncPer; ++u) {
-    const int i = blockIdx.x * kWireEncTile + u * kWireEncThreads + threadIdx.x;
-    const int slotix = u * kWireEncThreads + threadIdx.x;
+struct EpWireCodec {
+  using Params = EpWireEncodeParams;
+  using Msg = EpMsg;
+  static __device__ __forceinline__ bool stand_down(const Params& P) { return __ldcg(P.refused) != 0; }
+  static __device__ __forceinline__ Msg msg(const Params& P, int i, int* code) {
     bool bad = false;
-    EpMsg m{};
-    if (i < P.n) m = ep_enc_msg(P, i, &bad);
-    const uint32_t sz = i < P.n ? (uint32_t)ep_msg_size(m, P.replicas) : 0u;
-    uint32_t tot;
-    const uint32_t off = run + cta_scan<kWireEncThreads, true>(sz, ScanSum(), &tot);
-    run += tot;
-    s_len[slotix] = 0;
-    if (i < P.n) P.offs[i] = (int32_t)(gbase + off);
-    if (sz) {
-      uint8_t* p = P.out + gbase + off;
-      *p++ = (uint8_t)(m.member << 3 | 2);
-      p = wire_put_varint(p, (unsigned long long)ep_msg_body<false>(m, P.replicas, nullptr, nullptr));
-      uint8_t* vdst = nullptr;
-      ep_msg_body<true>(m, P.replicas, p, &vdst);
-      if (vdst) {
-        s_dst[slotix] = (uint32_t)(vdst - P.out);
-        s_src[slotix] = m.src;
-        s_len[slotix] = m.vlen;
-      }
-    }
+    const EpMsg m = ep_enc_msg(P, i, &bad);
+    if (bad) *code = FPX_ERR_INVALID_ARG;
+    return m;
   }
-  if (blockIdx.x == tiles - 1 && threadIdx.x == 0) P.offs[P.n] = (int32_t)(gbase + run);
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int m = warp; m < kWireEncTile; m += kWireEncThreads / 32) {
-    const int len = s_len[m];
-    const uint8_t* src = P.arena + s_src[m];
-    uint8_t* dst = P.out + s_dst[m];
-    for (int k = lane; k < len; k += 32) dst[k] = __ldg(src + k);
+  static __device__ __forceinline__ int size(const Params& P, const Msg& m) { return ep_msg_size(m, P.replicas); }
+  static __device__ __forceinline__ int size_of(const Params& P, int i, int* code) { return size(P, msg(P, i, code)); }
+  static __device__ __forceinline__ uint8_t* head(const Params& P, const Msg& m, uint8_t* p, int* gsrc, int* glen) {
+    *p++ = (uint8_t)(m.member << 3 | 2);
+    p = wire_put_varint(p, (unsigned long long)ep_msg_body<false>(m, P.replicas, nullptr, nullptr));
+    uint8_t* vdst = nullptr;
+    ep_msg_body<true>(m, P.replicas, p, &vdst);
+    if (!vdst) return p;
+    *gsrc = m.src; *glen = m.vlen;
+    return vdst;
   }
-}
+};
 
 }  // namespace fpx

@@ -12,11 +12,6 @@
 
 namespace fpx {
 
-// err_word of DevStatus and ReadsDev alike: min over errors of (index << 8 | -code)
-__device__ __forceinline__ void wire_reads_error(unsigned long long* err_word, int code, long long index) {
-  atomicMin(err_word, ((unsigned long long)index << 8) | (unsigned long long)(unsigned)(-code));
-}
-
 // The member that stands once the whole message is read (the last one on the wire) and the position of the first
 // occurrence of its final run: protobuf-java merges a member given again and drops it when another member follows.
 // Field numbers 1..members with wire type 2 are members; anything else is skipped as unknown.
@@ -124,7 +119,7 @@ struct RwEmit {
 };
 
 // The final run of member `which` from reader position `run` on, merged into m.  kEmit: one read record per Command.
-template <bool kS, bool kEmit>
+template <bool kEmit, bool kS>
 __device__ __forceinline__ bool rw_run(WireReader<kS> r, uint32_t run, int which, RwMsg& m, const RwEmit* o) {
   r.p = run;
   const int cf = rw_command_field(which);
@@ -219,17 +214,12 @@ __global__ void __launch_bounds__(kRwThreads) rw_count_kernel(RwDecodeParams P) 
   int kind = 0;
   RwMsg m{-1, 0, 0u, 0u, 0u};
   if (i < m1) {
-    const long long a = P.offs[i], b = P.offs[i + 1];
-    bool ok = w.sane && a <= b && a >= w.lo && b <= w.hi;      // offsets must be monotone
-    uint32_t run = 0, blo, bhi;
-    if (ok && w.staged) {
-      WireReader<true> r{(uint32_t)__cvta_generic_to_shared(s_buf), nullptr, (uint32_t)(a - w.base), (uint32_t)(b - w.base), true};
-      ok = wire_oneof_run(r, 7, &kind, &run, &blo, &bhi) && (kind == 0 || rw_run<true, false>(r, run, kind, m, nullptr));
-      m.voff += (uint32_t)w.base;                                 // window -> buffer offsets
-    } else if (ok) {
-      WireReader<false> r{0u, P.bytes, (uint32_t)a, (uint32_t)b, true};
-      ok = wire_oneof_run(r, 7, &kind, &run, &blo, &bhi) && (kind == 0 || rw_run<false, false>(r, run, kind, m, nullptr));
-    }
+    bool ok = false;
+    wire_read(w, s_buf, P.bytes, P.offs[i], P.offs[i + 1], [&](auto r, uint32_t rebase) {
+      uint32_t run = 0, blo, bhi;
+      ok = wire_oneof_run(r, 7, &kind, &run, &blo, &bhi) && (kind == 0 || rw_run<false>(r, run, kind, m, nullptr));
+      m.voff += rebase;
+    });
     if (!ok) {
       report_error(P.st, FPX_ERR_WIRE, i);
       kind = 0;
@@ -305,20 +295,14 @@ __global__ void __launch_bounds__(kRwThreads) rw_emit_kernel(RwDecodeParams P) {
     report_error(P.st, FPX_ERR_OVERFLOW_FULL, i);
     return;
   }
-  const long long a = P.offs[i], b = P.offs[i + 1];
-  if (!(w.sane && a <= b && a >= w.lo && b <= w.hi)) return;   // the count pass refused it already
-  RwMsg m{-1, 0, 0u, 0u, 0u};
-  int which;
-  uint32_t run, blo, bhi;
-  if (w.staged) {
-    WireReader<true> r{(uint32_t)__cvta_generic_to_shared(s_buf), nullptr, (uint32_t)(a - w.base), (uint32_t)(b - w.base), true};
-    const RwEmit o{P.reads, P.read_spans, (long long)off_r, cnt, __ldcg(&P.slot[i]), P.handle_base, (uint32_t)w.base};
-    if (wire_oneof_run(r, 7, &which, &run, &blo, &bhi)) rw_run<true, true>(r, run, which, m, &o);
-  } else {
-    WireReader<false> r{0u, P.bytes, (uint32_t)a, (uint32_t)b, true};
-    const RwEmit o{P.reads, P.read_spans, (long long)off_r, cnt, __ldcg(&P.slot[i]), P.handle_base, 0u};
-    if (wire_oneof_run(r, 7, &which, &run, &blo, &bhi)) rw_run<false, true>(r, run, which, m, &o);
-  }
+  // a message outside the span: the count pass refused it already
+  wire_read(w, s_buf, P.bytes, P.offs[i], P.offs[i + 1], [&](auto r, uint32_t rebase) {
+    RwMsg m{-1, 0, 0u, 0u, 0u};
+    int which;
+    uint32_t run, blo, bhi;
+    const RwEmit o{P.reads, P.read_spans, (long long)off_r, cnt, __ldcg(&P.slot[i]), P.handle_base, rebase};
+    if (wire_oneof_run(r, 7, &which, &run, &blo, &bhi)) rw_run<true>(r, run, which, m, &o);
+  });
 }
 
 // ---------------------------------------------------------------------------
@@ -388,26 +372,20 @@ __global__ void __launch_bounds__(kWireDecThreads) rd_wire_decode_kernel(RdDecod
   const WireSpan w = wire_stage_span(P.bytes, P.offs, P.n, m0, m1, s_buf);
   const int i = m0 + threadIdx.x;
   if (i >= m1) return;
-  const long long a = P.offs[i], b = P.offs[i + 1];
   const bool batcher = P.batcher != 0;
   int which = 0, pseudo = 0, id = 0;
   int v[4] = {0, 0, 0, 0};
-  uint32_t run = 0, blo = 0, bhi = 0;
-  bool ok = w.sane && a <= b && a >= w.lo && b <= w.hi;      // offsets must be monotone
-  uint32_t rebase = 0;
-  if (ok && w.staged) {
-    WireReader<true> r{(uint32_t)__cvta_generic_to_shared(s_buf), nullptr, (uint32_t)(a - w.base), (uint32_t)(b - w.base), true};
+  uint32_t blo = 0, bhi = 0, rebase = 0;
+  bool ok = false;
+  wire_read(w, s_buf, P.bytes, P.offs[i], P.offs[i + 1], [&](auto r, uint32_t base) {
+    uint32_t run = 0;
     ok = wire_oneof_run(r, batcher ? 4 : 5, &which, &run, &blo, &bhi) &&
          (which != 4 || rd_reply_run(r, run, batcher, v, &pseudo, &id));
-    rebase = (uint32_t)w.base;
-  } else if (ok) {
-    WireReader<false> r{0u, P.bytes, (uint32_t)a, (uint32_t)b, true};
-    ok = wire_oneof_run(r, batcher ? 4 : 5, &which, &run, &blo, &bhi) &&
-         (which != 4 || rd_reply_run(r, run, batcher, v, &pseudo, &id));
-  }
+    rebase = base;
+  });
   int4 rec = make_int4(-1, 0, 0, 0);
   if (!ok) {
-    wire_reads_error(P.err_word, FPX_ERR_WIRE, i);
+    report_error(P.err_word, FPX_ERR_WIRE, i);
     which = 0;
   } else if (which == 4) {
     // voter = group << 16 | acceptor; a field outside [0, 2^15) names no voter (-1: the tally's BAD_ACCEPTOR rule)
@@ -429,21 +407,15 @@ __global__ void __launch_bounds__(kWireDecThreads) rd_wire_decode_kernel(RdDecod
 // encoders: the acceptor's MaxSlotReply / BatchMaxSlotReply, and a completed read's ReadRequest / ReadRequestBatch
 // ---------------------------------------------------------------------------
 struct RdEncodeParams {
+  WireEnc enc;                // enc.src: the request batch (client_address) or the arena
   int32_t read_requests;      // 0: max-slot replies (kind[] + fpx_wire_rec), 1: read requests (fpx_read_slot)
   int32_t outer;              // read requests: the member's tag byte (0x12 read_request, 0x2a read_request_batch)
   const int32_t* kind;
   const int4* in;
-  int32_t n;
-  const uint8_t* src;         // gathered bytes: the request batch (client_address) or the arena
   int32_t src_len;            // max-slot replies: bytes in the request batch
   const int32_t* value_offs;  // read requests
   int32_t num_values;
   int32_t groups, per_group;  // max-slot replies: the voters of the config
-  uint8_t* out;
-  int32_t out_capacity;
-  int32_t* offs;              // n + 1
-  uint32_t* tile_sum;         // [tiles + 1]
-  unsigned long long* err_word;
 };
 
 // One message: outer tag, [CommandId{client_address = gathered, pseudo, id} as field 1], int32 fields
@@ -472,7 +444,7 @@ __device__ __forceinline__ RdMsg rd_enc_msg(const RdEncodeParams& P, int i, int*
   const int kind = P.kind[i];
   if (kind != 3 && kind != 4) return m;
   // the request's body: {0, 0, body_off, body_len} as fpx_wire_decode_inbound writes it
-  WireReader<false> b{0u, P.src, (uint32_t)r.z, (uint32_t)r.z + (uint32_t)r.w, true};
+  WireReader<false> b{0u, P.enc.src, (uint32_t)r.z, (uint32_t)r.z + (uint32_t)r.w, true};
   bool ok = r.z >= 0 && r.w >= 0 && (long long)r.z + r.w <= P.src_len;
   unsigned have = 0, cid = 0;
   uint32_t aoff = 0, alen = 0;
@@ -529,74 +501,31 @@ __device__ __forceinline__ int rd_msg_size(const RdMsg& m) {
   return 1 + wire_varint_size((unsigned long long)b) + b;
 }
 
-// pass 1: bytes per tile of kWireEncTile records
-__global__ void __launch_bounds__(kWireEncThreads) rd_wire_size_kernel(RdEncodeParams P) {
-  uint32_t sum = 0;
-  for (int u = 0; u < kWireEncPer; ++u) {
-    const int i = blockIdx.x * kWireEncTile + (int)threadIdx.x * kWireEncPer + u;
-    if (i < P.n) {
-      int code = FPX_OK;
-      const RdMsg m = rd_enc_msg(P, i, &code);
-      if (code != FPX_OK) wire_reads_error(P.err_word, code, i);
-      sum += (uint32_t)rd_msg_size(m);
+struct RdWireCodec {
+  using Params = RdEncodeParams;
+  using Msg = RdMsg;
+  static __device__ __forceinline__ bool stand_down(const Params&) { return false; }
+  static __device__ __forceinline__ Msg msg(const Params& P, int i, int* code) { return rd_enc_msg(P, i, code); }
+  static __device__ __forceinline__ int size(const Params&, const Msg& m) { return rd_msg_size(m); }
+  static __device__ __forceinline__ int size_of(const Params& P, int i, int* code) { return rd_msg_size(rd_enc_msg(P, i, code)); }
+  // the client_address inside the CommandId, else the arena's bytes as the body's tail
+  static __device__ __forceinline__ uint8_t* head(const Params&, const Msg& m, uint8_t* p, int* gsrc, int* glen) {
+    *p++ = (uint8_t)m.outer;
+    p = wire_put_varint(p, (unsigned long long)rd_msg_body(m));
+    uint8_t* gdst = nullptr;
+    if (m.cid) {
+      *p++ = 0x0a; p = wire_put_varint(p, (unsigned long long)rd_cid_body(m));
+      *p++ = 0x0a; p = wire_put_varint(p, (unsigned long long)m.glen);
+      gdst = p; p += m.glen;
+      p = wire_put_int32(p, 2, m.pseudo); p = wire_put_int32(p, 3, m.id);
     }
-  }
-  sum = cta_reduce<kWireEncThreads>(sum, ScanSum());
-  if (threadIdx.x == 0) P.tile_sum[blockIdx.x] = sum;
-}
-
-// pass 3 (after tile_offsets_kernel): heads by the record's thread, gathered bytes by the CTA's warps
-__global__ void __launch_bounds__(kWireEncThreads) rd_wire_emit_kernel(RdEncodeParams P) {
-  __shared__ uint32_t s_dst[kWireEncTile];
-  __shared__ int32_t s_src[kWireEncTile], s_len[kWireEncTile];
-  const uint32_t tiles = gridDim.x;
-  if (__ldcg(&P.tile_sum[tiles]) > (uint32_t)P.out_capacity) {   // output buffer too small
-    if (blockIdx.x == 0 && threadIdx.x == 0) wire_reads_error(P.err_word, FPX_ERR_INVALID_ARG, 0);
-    return;
-  }
-  const uint32_t gbase = __ldcg(&P.tile_sum[blockIdx.x]);
-  uint32_t run = 0;
-  for (int u = 0; u < kWireEncPer; ++u) {
-    const int i = blockIdx.x * kWireEncTile + u * kWireEncThreads + threadIdx.x;
-    const int slotix = u * kWireEncThreads + threadIdx.x;
-    int code = FPX_OK;
-    RdMsg m{};
-    if (i < P.n) m = rd_enc_msg(P, i, &code);
-    const uint32_t sz = i < P.n ? (uint32_t)rd_msg_size(m) : 0u;
-    uint32_t tot;
-    const uint32_t off = run + cta_scan<kWireEncThreads, true>(sz, ScanSum(), &tot);
-    run += tot;
-    s_len[slotix] = 0;
-    if (i < P.n) P.offs[i] = (int32_t)(gbase + off);
-    if (sz) {
-      uint8_t* p = P.out + gbase + off;
-      *p++ = (uint8_t)m.outer;
-      p = wire_put_varint(p, (unsigned long long)rd_msg_body(m));
-      uint8_t* gdst = nullptr;
-      if (m.cid) {
-        *p++ = 0x0a; p = wire_put_varint(p, (unsigned long long)rd_cid_body(m));
-        *p++ = 0x0a; p = wire_put_varint(p, (unsigned long long)m.glen);
-        gdst = p; p += m.glen;
-        p = wire_put_int32(p, 2, m.pseudo); p = wire_put_int32(p, 3, m.id);
-      }
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        if (k < m.nf) p = wire_put_int32(p, m.f1 + k, m.v[k]);
-      if (!m.cid) gdst = p;
-      s_dst[slotix] = (uint32_t)(gdst - P.out);
-      s_src[slotix] = m.src;
-      s_len[slotix] = m.glen;
-    }
+    for (int k = 0; k < 4; ++k)
+      if (k < m.nf) p = wire_put_int32(p, m.f1 + k, m.v[k]);
+    if (!m.cid) gdst = p;
+    *gsrc = m.src; *glen = m.glen;
+    return gdst;
   }
-  if (blockIdx.x == tiles - 1 && threadIdx.x == 0) P.offs[P.n] = (int32_t)(gbase + run);
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int k = warp; k < kWireEncTile; k += kWireEncThreads / 32) {
-    const int len = s_len[k];
-    const uint8_t* src = P.src + s_src[k];
-    uint8_t* dst = P.out + s_dst[k];
-    for (int j = lane; j < len; j += 32) dst[j] = __ldg(src + j);
-  }
-}
+};
 
 }  // namespace fpx

@@ -1,6 +1,7 @@
 """Device time of the EPaxos wire codec on BASELINE cfg4's traffic (f = 2, n = 5 replicas, 2^20 instances led round
-robin): decode the 838 860 PreAccepts replica 0 receives and pack them into fpx_epaxos_preaccept rows, and decode the
-PreAcceptOks replica 0 receives as a leader and pack them into fpx_epaxos_preacceptok rows.  The bytes are written by
+robin): decode the 838 860 PreAccepts replica 0 receives and pack them into fpx_epaxos_preaccept rows, encode its
+handlePreAccept replies (the PreAcceptOks it sends back), and decode the PreAcceptOks replica 0 receives as a leader
+and pack them into fpx_epaxos_preacceptok rows.  The bytes are written by
 Google's Python protobuf runtime (tests/golden/make_wire_ep_golden.py's descriptor pool), the decoded rows checked
 against the trace.  CUDA events on the handle's stream, inputs resident in HBM, L2 flushed by a 256 MB read between
 rounds, 3 warm-up + 10 timed rounds.  The card's name and power limit are read in the same run.
@@ -17,7 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from frankenpaxos_b200 import traces as T  # noqa: E402
-from frankenpaxos_b200.epaxos import CALL_PREACCEPT, CALL_PREACCEPTOK, EpaxosReplica  # noqa: E402
+from frankenpaxos_b200.epaxos import CALL_PREACCEPT, CALL_PREACCEPTOK, REPLY_OK, EpaxosReplica  # noqa: E402
 import wire_ep_oracle as W  # noqa: E402
 
 assert torch.cuda.is_available(), "this measurement needs the GPU"
@@ -76,13 +77,43 @@ def measure(name, raws, call, expect, local_deps=None):
             "decode": {"ms": dec_ms, "ms_std": dec_sd, "messages_per_s": m / (dec_ms * 1e-3),
                        "algorithmic_bytes": dec_bytes, "GB/s": dec_bytes / (dec_ms * 1e-3) / 1e9,
                        "kernels": "ep_wire_decode_kernel"},
-            "pack": {"ms": pack_ms, "ms_std": pack_sd, "kernels": "ep_wire_pack_kernel"}}
+            "pack": {"ms": pack_ms, "ms_std": pack_sd, "kernels": "ep_wire_pack_kernel"}}, d_out
 
 
 res = {"workload": "cfg4 (f = 2, 2^20 instances): replica 0's PreAccepts and PreAcceptOks"}
-res["preaccept"] = measure("PreAccept", W.preaccept_messages(G, pa, n), CALL_PREACCEPT, pa, pa[:, 6:6 + n])
-res["preacceptok"] = measure("PreAcceptOk", W.preacceptok_messages(G, ok, n), CALL_PREACCEPTOK, ok)
-res["encode"] = "not measured"
+res["preaccept"], pa_rows = measure("PreAccept", W.preaccept_messages(G, pa, n), CALL_PREACCEPT, pa, pa[:, 6:6 + n])
+res["preacceptok"], _ = measure("PreAcceptOk", W.preacceptok_messages(G, ok, n), CALL_PREACCEPTOK, ok)
+
+
+def measure_encode(d_in, m):
+    """handlePreAccept on the packed rows once, then its m replies to bytes (fpx_epaxos_wire_encode_dev)"""
+    d_reply = torch.empty((m, 4 + n), dtype=torch.int32, device=dev)
+    eng.preaccept_dev(d_in.data_ptr(), m, d_reply.data_ptr())
+    eng.sync()
+    arena, voffs = W.value_arena(m + 1)                    # the decoder's value ids: batch positions
+    d_arena, d_voffs = torch.from_numpy(arena).to(dev), torch.from_numpy(voffs.astype(np.int32)).to(dev)
+    cap = m * (128 + 14 * n) + 16
+    d_bytes = torch.empty(cap, dtype=torch.uint8, device=dev)
+    d_offs = torch.empty(m + 1, dtype=torch.int32, device=dev)
+
+    def enc():
+        eng.wire_encode_dev(CALL_PREACCEPT, d_in.data_ptr(), d_reply.data_ptr(), m, d_arena.data_ptr(),
+                            d_voffs.data_ptr(), len(voffs) - 1, d_bytes.data_ptr(), cap, d_offs.data_ptr())
+
+    enc_ms, enc_sd = timed(enc)
+    eng.sync()
+    lens = np.diff(d_offs.cpu().numpy())
+    kinds = d_reply[:, 0].cpu().numpy()
+    assert bool((kinds == REPLY_OK).all()) and bool((lens > 0).all())   # a PreAcceptOk for every PreAccept
+    total = int(lens.sum())
+    enc_bytes = 4 * m * (6 + 2 * n) + 4 * m * (4 + n) + total + 4 * (m + 1)   # rows in, bytes + offsets out
+    return {"messages": m, "wire_bytes": total, "bytes_per_message": total / m, "ms": enc_ms, "ms_std": enc_sd,
+            "messages_per_s": m / (enc_ms * 1e-3), "algorithmic_bytes": enc_bytes,
+            "GB/s": enc_bytes / (enc_ms * 1e-3) / 1e9,
+            "kernels": "wire_size_kernel<EpWireCodec> + tile_offsets_kernel + wire_gather_emit_kernel<EpWireCodec>"}
+
+
+res["encode"] = {"preacceptok_replies": measure_encode(pa_rows, len(pa))}
 q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
 res.update({"device": torch.cuda.get_device_name(0), "nvidia_smi": q.stdout.strip(),
             "l2": "256 MB buffer read between rounds"})

@@ -82,7 +82,8 @@ print(json.dumps({
     "wire_bytes": total, "bytes_per_message": total / n,
     "encode": {"ms": enc_ms, "ms_std": enc_sd, "messages_per_s": n / (enc_ms * 1e-3), "algorithmic_bytes": enc_bytes,
                "GB/s": enc_bytes / (enc_ms * 1e-3) / 1e9,
-               "kernels": "wire_size_kernel<kWireVmReply> + tile_offsets_kernel + wire_emit_valued_kernel<kWireVmReply>"},
+               "kernels": "wire_size_kernel<WireKindCodec<kWireVmReply>> + tile_offsets_kernel + "
+                          "wire_gather_emit_kernel<WireKindCodec<kWireVmReply>>"},
     "decode": {"ms": dec_ms, "ms_std": dec_sd, "messages_per_s": n / (dec_ms * 1e-3), "algorithmic_bytes": dec_bytes,
                "GB/s": dec_bytes / (dec_ms * 1e-3) / 1e9, "kernels": "wire_decode_kernel"},
     "device": torch.cuda.get_device_name(0), "nvidia_smi": q.stdout.strip(), "l2": "256 MB buffer read between rounds"}))
