@@ -32,6 +32,7 @@
 #include "fpx_tally.cuh"
 #include "fpx_vanilla.cuh"
 #include "fpx_wire.cuh"
+#include "fpx_wire_phase1.cuh"
 #include "fpx_wire_reads.cuh"
 
 using namespace fpx;
@@ -51,6 +52,7 @@ struct WireStage {
   WireBuf kind, rec, sender, out, arena, voffs, tiles;
   WireBuf aux;                         // EPaxos: the encoder's output rows, the pack's local deps
   WireBuf rw_scratch, rw_out;          // the replica decode's per-message and per-tile scratch, its host-form output
+  WireBuf p1_scratch, p1_out, spans;   // the leader's Phase 1: messages, entries, window; its host-form output; Phase2a spans
 };
 
 struct fpx_engine {
@@ -1307,3 +1309,4 @@ int fpx_snapshot_log(fpx_engine* e, int32_t first_slot, int32_t n_slots, int32_t
 #include "fpx_engine_f4.inc"
 #include "fpx_engine_reads.inc"
 #include "fpx_engine_wire_reads.inc"
+#include "fpx_engine_wire_phase1.inc"

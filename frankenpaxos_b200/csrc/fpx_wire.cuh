@@ -762,7 +762,8 @@ __device__ __forceinline__ uint8_t* wire_put_int32(uint8_t* p, int field, int v)
 // kWireMencius{Nack, P2bRange, ChosenRange}: compartmentalized Mencius (Mencius.proto) LeaderInbound.nack = 7,
 // ProxyLeaderInbound.phase2b_noop_range = 5 and ReplicaInbound.chosen_noop_range = 2.
 enum { kWirePhase2b = 0, kWireNack = 1, kWireChosen = 2, kWireMenciusPhase2b = 3, kWireVmReply = 4, kWireVmChosen = 5,
-       kWireVmPhase2a = 6, kWireVmSkip = 7, kWireMenciusNack = 8, kWireMenciusP2bRange = 9, kWireMenciusChosenRange = 10 };
+       kWireVmPhase2a = 6, kWireVmSkip = 7, kWireMenciusNack = 8, kWireMenciusP2bRange = 9, kWireMenciusChosenRange = 10,
+       kWirePhase2a = 11 };
 // the largest message of a small-record encoder (its shared-memory slot per record)
 __host__ __device__ constexpr int wire_small_max(int kind) {
   return kind == kWireNack || kind == kWireMenciusNack ? kWireMaxNack : kind == kWireMenciusP2bRange ? kWireMaxP2bRange
@@ -770,7 +771,8 @@ __host__ __device__ constexpr int wire_small_max(int kind) {
 }
 // encoders whose messages carry a value from the arena: size -> scan -> wire_gather_emit_kernel
 __host__ __device__ constexpr bool wire_gathers(int kind) {
-  return kind == kWireChosen || kind == kWireVmReply || kind == kWireVmChosen || kind == kWireVmPhase2a;
+  return kind == kWireChosen || kind == kWireVmReply || kind == kWireVmChosen || kind == kWireVmPhase2a ||
+         kind == kWirePhase2a;
 }
 
 // What every encoder's params hold (as their member `enc`): n records in, n messages out.
@@ -792,6 +794,10 @@ struct WireEncodeParams {
   int32_t num_values;
   int32_t servers;            // kWireVmPhase2a: sending_server = slot mod servers
   int32_t agroups;            // kWireMenciusP2bRange: acceptor_group_index = (dst >> 16) mod agroups
+  // kWirePhase2a: value_id v is the span spans[v - span_base] = {off, len} of enc.src[0 .. span_bytes), for
+  // v - span_base in [0, num_values); value_offs is not read
+  const int2* spans;
+  int32_t span_base, span_bytes;
 };
 
 // One message of a value-gathering encoder: outer oneof tag, int32 fields 1..nf, then (vfield != 0) the
@@ -827,6 +833,17 @@ __device__ __forceinline__ WireMsg wire_msg(const WireEncodeParams& P, int i, bo
     const int2 r = ((const int2*)P.in)[i];
     m.outer = 0x3a; m.nf = 1; m.f0 = r.x; m.vfield = 2; m.revocation = true;
     *bad = !wire_value(P, r.y, true, &m);
+  } else if (KIND == kWirePhase2a) {                // ProxyLeaderInbound{phase2a = 1 {slot, round, command_batch_or_noop}}
+    const int4 r = ((const int4*)P.in)[i];
+    m.outer = 0x0a; m.nf = 2; m.f0 = r.x; m.f1 = r.y; m.vfield = 3;
+    if (r.z == FPX_VALUE_NOOP) {
+      m.noop = true; m.vlen = 2;
+    } else {
+      const uint32_t k = (uint32_t)r.z - (uint32_t)P.span_base;
+      const int2 sp = k < (uint32_t)P.num_values ? P.spans[k] : make_int2(-1, -1);
+      *bad = sp.x < 0 || sp.y < 0 || (long long)sp.x + sp.y > P.span_bytes;
+      m.src = sp.x; m.vlen = sp.y;
+    }
   } else if (KIND == kWireVmPhase2a) {              // ServerInbound{phase2a = 4 {sending_server, slot, round, value}}
     const int4 r = ((const int4*)P.in)[i];
     const int owner = r.x % P.servers;

@@ -556,6 +556,79 @@ class Engine(_Handle):
         self._check(self._L.fpx_wire_encode_max_slot_replies_dev(self.h, d_bytes, n_bytes, d_kind, d_in, n, d_out,
                                                                  out_capacity, d_offsets))
 
+    def leader_phase1b_wire(self, round_, chosen_watermark, buf, offsets, value_id_base=0, out_capacity=None):
+        """Leader.handlePhase1b over LeaderInbound bytes in delivery order -> (complete, max_slot, records P2A,
+        spans[k, 2]): complete = the index of the message that completed the read quorum (-1: none yet, no records);
+        record k re-proposes slot chosen_watermark + k, value_id_base + k with its vote value at spans[k] in buf, or
+        VALUE_NOOP.  out_capacity defaults to the engine's slot capacity."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offsets = np.ascontiguousarray(offsets, dtype=np.int32)
+        n = len(offsets) - 1
+        cap = self.cfg.slot_capacity if out_capacity is None else out_capacity
+        out = np.zeros(max(cap, 1), dtype=P2A)
+        spans = np.zeros((max(cap, 1), 2), dtype=np.int32)
+        res = np.zeros(3, dtype=np.int32)
+        self._host_call(self._L.fpx_leader_phase1b_wire, round_, chosen_watermark, buf.ctypes.data if len(buf) else None,
+                        offsets.ctypes.data, n, value_id_base, out.ctypes.data, spans.ctypes.data, cap, res.ctypes.data)
+        k = int(res[2])
+        return int(res[0]), int(res[1]), out[:k].copy(), spans[:k].copy()
+
+    def leader_phase1b_wire_dev(self, round_, chosen_watermark, d_bytes, n_bytes, d_offsets, n, value_id_base, d_out,
+                                d_spans, out_capacity, d_result):
+        self._check(self._L.fpx_leader_phase1b_wire_dev(self.h, round_, chosen_watermark, d_bytes, n_bytes, d_offsets, n,
+                                                        value_id_base, d_out, d_spans, out_capacity, d_result))
+
+    def acceptor_phase1a_wire(self, buf, kind, recs, arena, value_offsets):
+        """Acceptor.handlePhase1a per decoded AcceptorInbound record (a = group << 16 | acceptor) of the request batch
+        buf -> (bytes, offsets[n+1]): a Phase1b (votes' values from arena / value_offsets, VALUE_NOOP the Noop) or a
+        Nack per Phase1a, a zero-length message for any other kind."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        kind = np.ascontiguousarray(kind, dtype=np.int32)
+        recs = np.ascontiguousarray(recs, dtype=WIRE_REC)
+        arena = np.ascontiguousarray(arena, dtype=np.uint8)
+        value_offsets = np.ascontiguousarray(value_offsets, dtype=np.int32)
+        n = len(recs)
+        # an info is at most 32 bytes of head plus its value, one per slot up to the acceptor's maxVotedSlot
+        longest = max(int(np.diff(value_offsets).max()) if len(value_offsets) > 1 else 0, 2)
+        cap = 16 + 16 * n
+        for i in np.nonzero(kind == 1)[0]:
+            g, a = int(recs["a"][i]) >> 16, int(recs["a"][i]) & 0xffff
+            if g < self.cfg.num_acceptor_groups and a < self.cfg.acceptors_per_group:
+                cap += 48 + (self.snapshot_acceptor(g, a)[1] + 1) * (32 + longest)
+        cap = min(cap, (1 << 31) - 1)
+        out = np.zeros(cap, dtype=np.uint8)
+        offs = np.zeros(n + 1, dtype=np.int32)
+        self._host_call(self._L.fpx_acceptor_phase1a_wire, buf.ctypes.data if len(buf) else None, len(buf),
+                        kind.ctypes.data, recs.ctypes.data, n, arena.ctypes.data if len(arena) else None,
+                        value_offsets.ctypes.data, len(value_offsets) - 1, out.ctypes.data, cap, offs.ctypes.data)
+        return out[:offs[n]].copy(), offs
+
+    def acceptor_phase1a_wire_dev(self, d_bytes, n_bytes, d_kind, d_in, n, d_arena, d_value_offsets, num_values, d_out,
+                                  out_capacity, d_offsets):
+        self._check(self._L.fpx_acceptor_phase1a_wire_dev(self.h, d_bytes, n_bytes, d_kind, d_in, n, d_arena,
+                                                          d_value_offsets, num_values, d_out, out_capacity, d_offsets))
+
+    def wire_encode_phase2a(self, recs, buf, spans, value_id_base=0):
+        """P2A records -> ProxyLeaderInbound{phase2a} bytes, offsets[n+1]: value_id v is buf[spans[v - base]], VALUE_NOOP
+        the Noop (leader_phase1b_wire's output as it is)."""
+        recs = np.ascontiguousarray(recs, dtype=P2A)
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        spans = np.ascontiguousarray(spans, dtype=np.int32).reshape(-1, 2)
+        k = recs["value_id"].astype(np.int64) - value_id_base
+        ok = (recs["value_id"] != VALUE_NOOP) & (k >= 0) & (k < len(spans))
+        cap = int(32 * len(recs) + spans[k[ok], 1].clip(0).sum()) + 16   # 32: the longest head
+        n = len(recs)
+        out = np.zeros(cap, dtype=np.uint8)
+        offs = np.zeros(n + 1, dtype=np.int32)
+        self._host_call(self._L.fpx_wire_encode_phase2a, recs.ctypes.data, n, buf.ctypes.data if len(buf) else None,
+                        len(buf), spans.ctypes.data, len(spans), value_id_base, out.ctypes.data, cap, offs.ctypes.data)
+        return out[:offs[n]].copy(), offs
+
+    def wire_encode_phase2a_dev(self, d_in, n, d_bytes, n_bytes, d_spans, num_spans, value_id_base, d_out, out_capacity,
+                                d_offsets):
+        self._check(self._L.fpx_wire_encode_phase2a_dev(self.h, d_in, n, d_bytes, n_bytes, d_spans, num_spans,
+                                                        value_id_base, d_out, out_capacity, d_offsets))
+
     # -- device-pointer calls (raw device addresses, asynchronous on self.stream)
     def proxyleader_arm_dev(self, d_in, n):
         self._check(self._L.fpx_proxyleader_arm_dev(self.h, d_in, n))

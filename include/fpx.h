@@ -1105,6 +1105,78 @@ int fpx_wire_encode_max_slot_replies(fpx_engine* e, const uint8_t* bytes, int32_
 int fpx_wire_encode_max_slot_replies_dev(fpx_engine* e, const uint8_t* d_bytes, int32_t n_bytes, const int32_t* d_kind,
                                          const fpx_wire_rec* d_in, int32_t n, uint8_t* d_out, int32_t out_capacity,
                                          int32_t* d_offsets);
+/* The acceptors' Phase 1 from bytes (Acceptor.handlePhase1a, S/multipaxos/Acceptor.scala:148-182), protocol
+ * FPX_MULTIPAXOS with shard_count 1, else FPX_ERR_UNSUPPORTED.  kind[] and in[] as fpx_wire_decode_inbound(
+ * FPX_WIRE_ACCEPTOR_INBOUND) writes them for the request batch bytes[0 .. n_bytes), with a = group << 16 | acceptor
+ * filled in by the caller; n <= 65535.  One message per record; per acceptor, in delivery order:
+ *   1 phase1a, round < the acceptor's round -> LeaderInbound{nack{round = the acceptor's round}};
+ *   1 phase1a, otherwise                    -> round = phase1a.round and LeaderInbound{phase1b{group_index,
+ *        acceptor_index, round, info*}}: one info {slot, vote_round, vote_value} per voted slot >= chosen_watermark,
+ *        ascending; the vote's value_id v is arena[value_offsets[v] .. value_offsets[v+1]) (a CommandBatchOrNoop),
+ *        FPX_VALUE_NOOP the Noop (12 00); any other value_id is FPX_ERR_INVALID_ARG at the record;
+ *   any other kind                          -> a zero-length message, nothing changed (a Phase1a is a batch boundary
+ *        of the Phase2a stream, SURVEY 8(g) rule 2).
+ * A body that does not parse or lacks a required field is FPX_ERR_WIRE at its record, a voter that names no acceptor
+ * FPX_ERR_INVALID_ARG, a chosen_watermark below the first slot the engine still holds after fpx_retire_below (whose
+ * votes it no longer has) FPX_ERR_SLOT_RANGE; with any of these no round changes.  Afterwards the rounds are what
+ * fpx_acceptor_phase1a would have left.  out_capacity as for the encoders above.  Both forms read the info count back
+ * once (it sizes the encoder): the _dev form synchronises the engine's stream. */
+int fpx_acceptor_phase1a_wire(fpx_engine* e, const uint8_t* bytes, int32_t n_bytes, const int32_t* kind,
+                              const fpx_wire_rec* in, int32_t n, const uint8_t* arena, const int32_t* value_offsets,
+                              int32_t num_values, uint8_t* out, int32_t out_capacity, int32_t* offsets,
+                              int64_t* err_index);
+int fpx_acceptor_phase1a_wire_dev(fpx_engine* e, const uint8_t* d_bytes, int32_t n_bytes, const int32_t* d_kind,
+                                  const fpx_wire_rec* d_in, int32_t n, const uint8_t* d_arena,
+                                  const int32_t* d_value_offsets, int32_t num_values, uint8_t* d_out,
+                                  int32_t out_capacity, int32_t* d_offsets);
+/* ---- The new leader's Phase 1 from bytes (Leader.handlePhase1b, S/multipaxos/Leader.scala:504-577) ---------------
+ * Protocol FPX_MULTIPAXOS with shard_count 1, else FPX_ERR_UNSUPPORTED.  The call is stateless: the engine supplies the
+ * geometry (f, groups, grid) and its stream, and holds no leader state.  bytes / offsets[n+1]: the LeaderInbound
+ * messages (MultiPaxos.proto:525-539; Phase1b :263-271, Phase1bSlotInfo :254-261) received since Phase 1 began, in
+ * delivery order; parsing rules as for the wire codec above.  The Phase1b's bodies and its info entries are parsed;
+ * the body of any other member is skipped by length, not parsed; a phase1b member given again merges (info appends,
+ * a later scalar wins), another member replaces it.  A second vote_value in one info is FPX_ERR_WIRE (protobuf would
+ * merge the two CommandBatchOrNoops), like a second command_batch_or_noop above.  Per message, in delivery order:
+ *   malformed bytes or a missing required field       -> FPX_ERR_WIRE at the message;
+ *   not a phase1b                                      -> skipped;
+ *   phase1b.round < round                              -> ignored (:517-525);
+ *   phase1b.round > round                              -> FPX_ERR_CHECK_FAILED at the message (logger.checkLt);
+ *   group_index / acceptor_index outside the config    -> FPX_ERR_BAD_ACCEPTOR at the message;
+ *   else phase1bs(group)(acceptor) = the message (a later Phase1b of an acceptor replaces its earlier one); the quorum
+ *   completes when every group holds f+1 acceptors (flexible: Grid.isReadQuorum over the holders).
+ * result[0] = complete, the index of the completing message, or -1: then nothing is emitted and the caller calls again
+ * with more messages.  Messages after `complete` are not read.  result[1] = max_slot, the largest info slot of the
+ * Phase1bs held at completion (maxPhase1bSlot, -1 for none), result[2] = n_out = max(0, max_slot - chosen_watermark +
+ * 1).  Record k of out is Phase2a{slot = chosen_watermark + k, round, safeValue(phase1bs(slot % num_acceptor_groups),
+ * slot)} as {slot, round, value_id, -1}: value_id = value_id_base + k where a holder voted (spans[2k..2k+1] = {off, len}
+ * of its vote_value in bytes), FPX_VALUE_NOOP where none did (spans {0, 0}).  safeValue takes the first info of the
+ * slot in each Phase1b (info.find) and the highest vote_round; ties in vote_round, which correct acceptors never
+ * produce, go to the lowest acceptor index (DESIGN.md §7, beside the EPaxos recovery tie rule).  The records go
+ * to fpx_proxyleader_arm as they are.  More than out_capacity records: FPX_ERR_INVALID_ARG at `complete` and nothing
+ * written.  chosen_watermark < 0: FPX_ERR_INVALID_ARG.  Unlike fpx_leader_safe_values this reads the Phase1bs, so on a
+ * flexible grid it is the reference's fill-in exactly: one grid row per slot.  The call's device scratch is about
+ * 2 x the batch's bytes (one entry per 8 bytes) plus out_capacity x acceptors_per_group x 4 bytes (the info.find
+ * window, cleared on every call): out_capacity is best the largest window the caller expects, not a "no limit".
+ * _dev: d_bytes holds n_bytes bytes (offsets[n] - offsets[0] beyond them is FPX_ERR_WIRE at the message that reaches
+ * past them); d_result is a device int32[3] written on the stream; the status and first index are collected by
+ * fpx_sync; d_spans is 8-byte aligned. */
+int fpx_leader_phase1b_wire(fpx_engine* e, int32_t round, int32_t chosen_watermark, const uint8_t* bytes,
+                            const int32_t* offsets, int32_t n, int32_t value_id_base, fpx_p2a* out, int32_t* spans,
+                            int32_t out_capacity, int32_t* result, int64_t* err_index);
+int fpx_leader_phase1b_wire_dev(fpx_engine* e, int32_t round, int32_t chosen_watermark, const uint8_t* d_bytes,
+                                int32_t n_bytes, const int32_t* d_offsets, int32_t n, int32_t value_id_base,
+                                fpx_p2a* d_out, int32_t* d_spans, int32_t out_capacity, int32_t* d_result);
+/* ProxyLeaderInbound{phase2a{slot, round, command_batch_or_noop}} per fpx_p2a record (dst is not on the wire):
+ * value_id v is bytes[spans[2k] .. spans[2k] + spans[2k+1]) for k = v - value_id_base in [0, num_spans), FPX_VALUE_NOOP
+ * is CommandBatchOrNoop{noop {}} (12 00); anything else, or a span outside bytes[0 .. n_bytes), is FPX_ERR_INVALID_ARG
+ * at the record.  With fpx_leader_phase1b_wire's output: the Phase1b batch as bytes, its spans and value_id_base.
+ * Protocol FPX_MULTIPAXOS with shard_count 1, else FPX_ERR_UNSUPPORTED; out_capacity as for the encoders above. */
+int fpx_wire_encode_phase2a(fpx_engine* e, const fpx_p2a* in, int32_t n, const uint8_t* bytes, int32_t n_bytes,
+                            const int32_t* spans, int32_t num_spans, int32_t value_id_base, uint8_t* out,
+                            int32_t out_capacity, int32_t* offsets, int64_t* err_index);
+int fpx_wire_encode_phase2a_dev(fpx_engine* e, const fpx_p2a* d_in, int32_t n, const uint8_t* d_bytes, int32_t n_bytes,
+                                const int32_t* d_spans, int32_t num_spans, int32_t value_id_base, uint8_t* d_out,
+                                int32_t out_capacity, int32_t* d_offsets);
 /* The replies a Client or ReadBatcher receives, by the handle's kind; out[] goes to fpx_reads_max_slot_replies[_dev]
  * as it is, spans[2i..2i+1] = {off, len} of the member's body (its last occurrence), {0, 0} for no member.
  *   FPX_READS_CLIENT, ClientInbound: max_slot_reply (4) -> {key = client_pseudonym, id = client_id,
