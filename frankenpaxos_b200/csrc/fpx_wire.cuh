@@ -760,10 +760,11 @@ __device__ __forceinline__ uint8_t* wire_put_int32(uint8_t* p, int field, int v)
 // kWireVm*: vanilla Mencius ServerInbound (VanillaMencius.proto:227-241).  kWireVmReply is the dense reply
 // stream of fpx_vm_phase2a (fpx_p2b {kind, server, slot, round|value}), one message per record by its kind.
 // kWireMencius{Nack, P2bRange, ChosenRange}: compartmentalized Mencius (Mencius.proto) LeaderInbound.nack = 7,
-// ProxyLeaderInbound.phase2b_noop_range = 5 and ReplicaInbound.chosen_noop_range = 2.
+// ProxyLeaderInbound.phase2b_noop_range = 5 and ReplicaInbound.chosen_noop_range = 2.  kWireMenciusPhase2a is
+// kWirePhase2a under Mencius' ProxyLeaderInbound.phase2a = 2.
 enum { kWirePhase2b = 0, kWireNack = 1, kWireChosen = 2, kWireMenciusPhase2b = 3, kWireVmReply = 4, kWireVmChosen = 5,
        kWireVmPhase2a = 6, kWireVmSkip = 7, kWireMenciusNack = 8, kWireMenciusP2bRange = 9, kWireMenciusChosenRange = 10,
-       kWirePhase2a = 11 };
+       kWirePhase2a = 11, kWireMenciusPhase2a = 12 };
 // the largest message of a small-record encoder (its shared-memory slot per record)
 __host__ __device__ constexpr int wire_small_max(int kind) {
   return kind == kWireNack || kind == kWireMenciusNack ? kWireMaxNack : kind == kWireMenciusP2bRange ? kWireMaxP2bRange
@@ -772,7 +773,7 @@ __host__ __device__ constexpr int wire_small_max(int kind) {
 // encoders whose messages carry a value from the arena: size -> scan -> wire_gather_emit_kernel
 __host__ __device__ constexpr bool wire_gathers(int kind) {
   return kind == kWireChosen || kind == kWireVmReply || kind == kWireVmChosen || kind == kWireVmPhase2a ||
-         kind == kWirePhase2a;
+         kind == kWirePhase2a || kind == kWireMenciusPhase2a;
 }
 
 // What every encoder's params hold (as their member `enc`): n records in, n messages out.
@@ -833,9 +834,10 @@ __device__ __forceinline__ WireMsg wire_msg(const WireEncodeParams& P, int i, bo
     const int2 r = ((const int2*)P.in)[i];
     m.outer = 0x3a; m.nf = 1; m.f0 = r.x; m.vfield = 2; m.revocation = true;
     *bad = !wire_value(P, r.y, true, &m);
-  } else if (KIND == kWirePhase2a) {                // ProxyLeaderInbound{phase2a = 1 {slot, round, command_batch_or_noop}}
+  } else if (KIND == kWirePhase2a || KIND == kWireMenciusPhase2a) {
+    // ProxyLeaderInbound{phase2a = 1 (Mencius 2) {slot, round, command_batch_or_noop}}
     const int4 r = ((const int4*)P.in)[i];
-    m.outer = 0x0a; m.nf = 2; m.f0 = r.x; m.f1 = r.y; m.vfield = 3;
+    m.outer = KIND == kWirePhase2a ? 0x0a : 0x12; m.nf = 2; m.f0 = r.x; m.f1 = r.y; m.vfield = 3;
     if (r.z == FPX_VALUE_NOOP) {
       m.noop = true; m.vlen = 2;
     } else {

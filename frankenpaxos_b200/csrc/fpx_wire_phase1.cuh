@@ -1,4 +1,5 @@
-// fpx_wire_phase1.cuh -- the new leader's Phase 1 from protobuf bytes (include/fpx.h fpx_leader_phase1b_wire).
+// fpx_wire_phase1.cuh -- the new leader's Phase 1 from protobuf bytes (include/fpx.h fpx_leader_phase1b_wire and
+// fpx_mencius_leader_phase1b_wire).
 //
 // S/multipaxos/MultiPaxos.proto: Phase1bSlotInfo :254-261, Phase1b :263-271, LeaderInbound :525-539 (phase1b = 1 of
 // eight members).  Leader.handlePhase1b (S/multipaxos/Leader.scala:504-577) stores the Phase1bs of the leader's round
@@ -16,6 +17,11 @@
 //           [slot - chosen_watermark][acceptor index] window.
 //   emit    one thread per slot of [chosen_watermark, max_slot]: the arg-max over {vote_round, lowest acceptor} of
 //           that window row, written as an fpx_p2a record and the vote value's span.
+// Compartmentalized Mencius (S/mencius/Leader.scala:582-659) runs the same passes for one leader group: LeaderInbound
+// has nine members, the quorum is f+1 in each of the group's AG acceptor groups, max_slot is seeded with recoverSlot
+// and must be owned by the group, and the slots re-proposed are s0 = nextClassicRound(leader_group, chosenWatermark - 1)
+// to max_slot by LG, slot s read from acceptor group (s / LG) % AG.  MultiPaxos is that with LG = 1, leader_group 0 and
+// no recoverSlot: s0 = chosen_watermark, stride 1, group s % G.  The window row of slot s is (s - s0) / LG.
 #pragma once
 #include "fpx_wire.cuh"
 
@@ -40,12 +46,15 @@ struct P1Params {
   const int32_t* offs;                 // n + 1
   int32_t n, n_bytes;
   int32_t round, chosen_watermark, value_id_base, out_capacity;
-  int32_t groups, per_group, flexible, quorum;
+  int32_t groups, per_group, flexible, quorum;  // Mencius: groups = AG, the acceptor groups of one leader group
+  int32_t mencius, lgroups, leader_group;  // MultiPaxos: 0, 1, 0
+  int32_t recover_slot;                // seeds max_slot; MultiPaxos INT_MIN (no seed)
+  long long s0;                        // the first slot re-proposed; MultiPaxos chosen_watermark
   P1Msg* msg;                          // n
   int4* ent;                           // walk: {body off, body len, -, -}; parse: {slot, vote_round, value off, len}
   int32_t* sel;                        // [groups * per_group]: the message held as phase1bs(g)(a), -1 none
   int32_t* first;                      // [out_capacity * per_group], kP1NoEntry
-  int32_t* res;                        // {complete, max_slot, n_out}
+  int32_t* res;                        // {complete, max_slot, n_out}, Mencius and next_slot
   fpx_p2a* out;
   int2* spans;
   unsigned long long* err_word;
@@ -74,7 +83,9 @@ __device__ __forceinline__ uint32_t p1_varint(const uint8_t* w, long long wb, lo
 }
 
 // Walk: one CTA per message.  Thread 0 keeps the walker's state across the window steps; a step stops when the next
-// field header (at most 20 bytes: a tag and a ten-byte varint) may cross the window's end.
+// field header (at most 20 bytes: a tag and a ten-byte varint) may cross the window's end.  MEMBERS: LeaderInbound's
+// oneof members, 8 (MultiPaxos) or 9 (Mencius) -- a constant in the per-entry loop.
+template <int MEMBERS>
 __global__ void __launch_bounds__(kP1Threads) p1_walk_kernel(P1Params P) {
   __shared__ __align__(16) uint8_t s_win[kP1Window];
   __shared__ long long s_wb;
@@ -125,7 +136,7 @@ __global__ void __launch_bounds__(kP1Threads) p1_walk_kernel(P1Params P) {
         } else if (wt == 2) {
           v = p1_varint(s_win, wb, p, lim, ok, &h);
           if (!ok || h || (v >> 31) || lim - p < (long long)v) { ok = false; break; }
-          if (level == 0 && f <= 8) {
+          if (level == 0 && f <= MEMBERS) {
             // oneof: another member replaces the one before; the same member again merges into it
             if (f == 1) {
               if (r.kind != 1) { r.round = r.group = r.acceptor = 0; r.n_info = 0; have = 0; short_info = false; }
@@ -213,7 +224,7 @@ __device__ __forceinline__ bool p1_complete(const P1Params& P, uint32_t mask) {
   return !P.flexible;
 }
 
-// Select: the messages in delivery order, one thread.  res = {complete, max_slot seed, 0}.
+// Select: the messages in delivery order, one thread.  res = {complete, max_slot seed, 0(, -1)}.
 __global__ void p1_select_kernel(P1Params P) {
   const int keys = P.groups * P.per_group;
   for (int k = 0; k < keys; ++k) P.sel[k] = -1;
@@ -240,8 +251,9 @@ __global__ void p1_select_kernel(P1Params P) {
     for (int k = 0; k < keys; ++k)
       if (P.sel[k] >= 0 && P.msg[P.sel[k]].n_info == 0) seed = -1;
   P.res[0] = complete;
-  P.res[1] = complete >= 0 ? seed : -1;
+  P.res[1] = complete >= 0 ? max(seed, P.recover_slot) : -1;   // Mencius: max(..., phase1.recoverSlot)
   P.res[2] = 0;
+  if (P.mencius) P.res[3] = -1;
 }
 
 // the entries of the Phase1bs held at completion: f(entry, message)
@@ -267,11 +279,31 @@ __global__ void __launch_bounds__(kP1Threads) p1_max_kernel(P1Params P) {
   if ((threadIdx.x & 31) == 0 && mx != INT_MIN) atomicMax(&P.res[1], mx);
 }
 
-// the window [chosen_watermark, max_slot] when the call completes and the records fit, else 0 slots
+// the slots s0, s0 + LG, ... up to max_slot
+__device__ __forceinline__ long long p1_count(const P1Params& P, long long max_slot) {
+  return max_slot >= P.s0 ? (max_slot - P.s0) / P.lgroups + 1 : 0;
+}
+// Mencius: nextSlot = nextClassicRound(leader_group, max_slot) (RoundSystem.scala:66-80), in 64 bits
+__device__ __forceinline__ long long p1_next_slot(const P1Params& P, long long max_slot) {
+  if (max_slot < 0) return P.leader_group;
+  const long long base = P.lgroups * (max_slot / P.lgroups) + P.leader_group;
+  return base > max_slot ? base : base + P.lgroups;
+}
+// why a completed call emits nothing (FPX_OK: it emits): the Mencius max_slot owner check (logger.check), a
+// next_slot past int32, then more records than out_capacity
+__device__ __forceinline__ int p1_refusal(const P1Params& P, long long max_slot) {
+  if (P.mencius) {
+    if (max_slot != -1 && max_slot % P.lgroups != P.leader_group) return FPX_ERR_CHECK_FAILED;
+    if (p1_next_slot(P, max_slot) > INT_MAX) return FPX_ERR_SLOT_RANGE;
+  }
+  return p1_count(P, max_slot) > P.out_capacity ? FPX_ERR_INVALID_ARG : FPX_OK;
+}
+
+// the window rows [0, count) when the call completes and emits, else 0 rows
 __device__ __forceinline__ long long p1_window(const P1Params& P) {
   if (__ldcg(&P.res[0]) < 0) return 0;
-  const long long count = (long long)__ldcg(&P.res[1]) - P.chosen_watermark + 1;
-  return count > 0 && count <= P.out_capacity ? count : 0;
+  const long long max_slot = __ldcg(&P.res[1]);
+  return p1_refusal(P, max_slot) == FPX_OK ? p1_count(P, max_slot) : 0;
 }
 
 __global__ void __launch_bounds__(kP1Threads) p1_first_kernel(P1Params P) {
@@ -279,9 +311,12 @@ __global__ void __launch_bounds__(kP1Threads) p1_first_kernel(P1Params P) {
   if (count == 0) return;
   p1_for_held(P, [&](long long e, const P1Msg& r) {
     const int slot = P.ent[e].x;
-    const long long k = (long long)slot - P.chosen_watermark;
-    // safeValue reads phase1bs(slot % numAcceptorGroups) only (:552)
-    if (k < 0 || k >= count || slot % P.groups != r.group) return;
+    const long long d = (long long)slot - P.s0;               // < 2^31 once it is >= 0
+    // a slot of another leader group counts toward max_slot only
+    if (d < 0 || (uint32_t)d % (uint32_t)P.lgroups != 0) return;
+    const long long k = (uint32_t)d / (uint32_t)P.lgroups;
+    // safeValue reads phase1bs(slot % numAcceptorGroups) only (:552); Mencius acceptorGroupIndexBySlot (:342-345)
+    if (k >= count || (slot / P.lgroups) % P.groups != r.group) return;
     atomicMin(&P.first[k * P.per_group + r.acceptor], (int32_t)e);
   });
 }
@@ -289,13 +324,17 @@ __global__ void __launch_bounds__(kP1Threads) p1_first_kernel(P1Params P) {
 __global__ void __launch_bounds__(kP1Threads) p1_emit_kernel(P1Params P) {
   const int complete = __ldcg(&P.res[0]);
   if (complete < 0) return;
-  const long long want = (long long)__ldcg(&P.res[1]) - P.chosen_watermark + 1;
-  if (want > P.out_capacity) {                                  // refused: nothing written
-    if (blockIdx.x == 0 && threadIdx.x == 0) report_error(P.err_word, FPX_ERR_INVALID_ARG, complete);
+  const long long max_slot = __ldcg(&P.res[1]);
+  const int refused = p1_refusal(P, max_slot);
+  if (refused != FPX_OK) {                                      // nothing written
+    if (blockIdx.x == 0 && threadIdx.x == 0) report_error(P.err_word, refused, complete);
     return;
   }
-  const long long count = want > 0 ? want : 0;
-  if (blockIdx.x == 0 && threadIdx.x == 0) P.res[2] = (int32_t)count;
+  const long long count = p1_count(P, max_slot);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    P.res[2] = (int32_t)count;
+    if (P.mencius) P.res[3] = (int32_t)p1_next_slot(P, max_slot);
+  }
   for (long long k = (long long)blockIdx.x * kP1Threads + threadIdx.x; k < count; k += (long long)gridDim.x * kP1Threads) {
     int best = -1, bvr = 0;
     for (int a = 0; a < P.per_group; ++a) {                    // ties in vote_round: the lowest acceptor index
@@ -304,7 +343,7 @@ __global__ void __launch_bounds__(kP1Threads) p1_emit_kernel(P1Params P) {
       const int vr = P.ent[e].y;
       if (best < 0 || vr > bvr) { best = e; bvr = vr; }
     }
-    const int slot = (int)(P.chosen_watermark + k);
+    const int slot = (int)(P.s0 + k * P.lgroups);
     int2 sp = make_int2(0, 0);
     int value = FPX_VALUE_NOOP;
     if (best >= 0) {
@@ -329,6 +368,10 @@ __global__ void __launch_bounds__(kP1Threads) p1_emit_kernel(P1Params P) {
 //   fill    (slot tile, record): one encode record per message header and per info, and the message's summed
 //           body length (atomicAdd) which the header needs;
 //   encode  the gathering encoder with P1bCodec over the n + infos records, then the messages' offsets.
+// Compartmentalized Mencius (S/mencius/Acceptor.scala:166-200, fpx_mencius_acceptor_phase1a_wire) differs in what the
+// passes read and write, not in the passes: acceptor (lg, ag) holds the slots lg + LG * ag mod LG * AG, so count and
+// fill step by LG * AG from the first such slot >= chosen_watermark, up to the end of the live window (its
+// Phase2aNoopRange votes do not raise acc_max_voted); the Phase1b's group_index is ag and the Nack is member 7.
 // ---------------------------------------------------------------------------
 constexpr int kP1aTile = 1024;       // slots per count / fill CTA (4 per thread)
 enum { kP1aNone = 0, kP1aPhase1b = 1, kP1aNack = 2 };
@@ -354,6 +397,10 @@ struct P1aParams {
   const int32_t* value_offs;
   int32_t num_values;
   unsigned long long* err_word;
+  int32_t mencius;                     // slots of the acceptor's residue, to the live window's end
+  int32_t stride;                      // 1, Mencius LG * AG
+  int32_t wire_groups;                 // Phase1b.group_index = engine group % wire_groups (Mencius AG)
+  int32_t nack_tag;                    // LeaderInbound.nack: 0x32 (= 6), Mencius 0x3a (= 7)
 };
 
 // (vote round, value) of acceptor (group, acceptor) at slot, round -1 for none (fpx_snapshot_acceptor's rule)
@@ -430,12 +477,21 @@ __global__ void p1a_apply_kernel(P1aParams P) {
   if (touched) P.acc_round[k] = cur;
 }
 
-// the Phase1b of record i covers slots [lo, hi]; tile t of it
+// the Phase1b of record i covers slots lo, lo + stride, ... <= hi; tile t of it
 __device__ __forceinline__ bool p1a_range(const P1aParams& P, int i, int* lo, int* hi) {
   if (__ldcg(P.bad) || P.reply[i] != kP1aPhase1b) return false;
   const int a = P.in[i].x;
   *lo = P.lo[i];
-  *hi = P.acc_max_voted[(a >> 16) * P.g.per_group + (a & 0xffff)];
+  if (P.mencius) {
+    // the first slot >= lo of the acceptor's residue lg + LG * ag; noop-range votes leave acc_max_voted as it was
+    const int group = a >> 16, r = group / P.g.agroups + P.g.lgroups * (group % P.g.agroups);
+    const long long first = (long long)*lo + ((r - *lo % P.stride) % P.stride + P.stride) % P.stride;
+    *hi = P.g.slot_capacity - 1;
+    if (first > *hi) return false;
+    *lo = (int)first;
+  } else {
+    *hi = P.acc_max_voted[(a >> 16) * P.g.per_group + (a & 0xffff)];
+  }
   return *lo <= *hi;
 }
 
@@ -446,7 +502,7 @@ __global__ void __launch_bounds__(256) p1a_count_kernel(P1aParams P) {
   if (p1a_range(P, i, &lo, &hi)) {
     const int a = P.in[i].x;
     for (int u = 0; u < kP1aTile / 256; ++u) {
-      const long long s = (long long)lo + (long long)t * kP1aTile + u * 256 + threadIdx.x;
+      const long long s = (long long)lo + ((long long)t * kP1aTile + u * 256 + threadIdx.x) * P.stride;
       int v;
       if (s <= hi && p1a_vote(P, a >> 16, a & 0xffff, (int)s, &v) >= 0) ++c;
     }
@@ -478,7 +534,7 @@ __global__ void __launch_bounds__(256) p1a_fill_kernel(P1aParams P) {
   uint32_t base = P.cnt[(long long)i * P.tiles + t];
   uint32_t sum = 0;
   for (int u = 0; u < kP1aTile / 256; ++u) {
-    const long long s = (long long)lo + (long long)t * kP1aTile + u * 256 + threadIdx.x;
+    const long long s = (long long)lo + ((long long)t * kP1aTile + u * 256 + threadIdx.x) * P.stride;
     int v = 0, vr = -1;
     if (live && s <= hi) vr = p1a_vote(P, a >> 16, a & 0xffff, (int)s, &v);
     uint32_t tot;
@@ -521,7 +577,7 @@ struct P1bCodec {
       if (rep == kP1aNack) { m.kind = 2; m.f0 = P.A.nack[i]; }
       else if (rep == kP1aPhase1b) {
         const int a = P.A.in[i].x;
-        m.kind = 1; m.f0 = a >> 16; m.f1 = a & 0xffff; m.f2 = P.A.rnd[i]; m.body = __ldcg(&P.A.body[i]);
+        m.kind = 1; m.f0 = (a >> 16) % P.A.wire_groups; m.f1 = a & 0xffff; m.f2 = P.A.rnd[i]; m.body = __ldcg(&P.A.body[i]);
       }
       return m;
     }
@@ -543,14 +599,14 @@ struct P1bCodec {
     return 0;
   }
   static __device__ __forceinline__ int size_of(const Params& P, int r, int* code) { return size(P, msg(P, r, code)); }
-  static __device__ __forceinline__ uint8_t* head(const Params&, const Msg& m, uint8_t* p, int* gsrc, int* glen) {
+  static __device__ __forceinline__ uint8_t* head(const Params& P, const Msg& m, uint8_t* p, int* gsrc, int* glen) {
     *gsrc = 0; *glen = 0;
     if (m.kind == 1) {                 // LeaderInbound{phase1b = 1 {group_index, acceptor_index, round, info...}}
       const int b = 3 + wire_int32_size(m.f0) + wire_int32_size(m.f1) + wire_int32_size(m.f2) + m.body;
       *p++ = 0x0a; p = wire_put_varint(p, (unsigned long long)b);
       p = wire_put_int32(p, 1, m.f0); p = wire_put_int32(p, 2, m.f1); p = wire_put_int32(p, 3, m.f2);
-    } else if (m.kind == 2) {          // LeaderInbound{nack = 6 {round}}
-      *p++ = 0x32; *p++ = (uint8_t)(1 + wire_int32_size(m.f0));
+    } else if (m.kind == 2) {          // LeaderInbound{nack = 6 (Mencius 7) {round}}
+      *p++ = (uint8_t)P.A.nack_tag; *p++ = (uint8_t)(1 + wire_int32_size(m.f0));
       p = wire_put_int32(p, 1, m.f0);
     } else if (m.kind == 3) {          // info = 4 {slot, vote_round, vote_value}
       const int b = 2 + wire_int32_size(m.f0) + wire_int32_size(m.f1) + 1 + wire_varint_size((unsigned long long)m.body) + m.body;

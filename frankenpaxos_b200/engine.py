@@ -629,6 +629,81 @@ class Engine(_Handle):
         self._check(self._L.fpx_wire_encode_phase2a_dev(self.h, d_in, n, d_bytes, n_bytes, d_spans, num_spans,
                                                         value_id_base, d_out, out_capacity, d_offsets))
 
+    def mencius_acceptor_phase1a_wire(self, buf, kind, recs, arena, value_offsets):
+        """Compartmentalized Mencius' Acceptor.handlePhase1a per decoded AcceptorInbound record (a = engine_group << 16
+        | acceptor) -> (bytes, offsets[n+1]): a Phase1b (group_index = engine_group % AG, Phase2a and noop-range
+        votes alike) or a Nack (member 7) per Phase1a, a zero-length message for any other kind."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        kind = np.ascontiguousarray(kind, dtype=np.int32)
+        recs = np.ascontiguousarray(recs, dtype=WIRE_REC)
+        arena = np.ascontiguousarray(arena, dtype=np.uint8)
+        value_offsets = np.ascontiguousarray(value_offsets, dtype=np.int32)
+        n = len(recs)
+        # an info is at most 32 bytes of head plus its value, one per slot of the acceptor's residue in the live window
+        longest = max(int(np.diff(value_offsets).max()) if len(value_offsets) > 1 else 0, 2)
+        held = self.cfg.slot_capacity // (max(self.cfg.num_leader_groups, 1) * self.cfg.num_acceptor_groups) + 1
+        cap = min(16 + 16 * n + int((kind == 1).sum()) * (48 + held * (32 + longest)), (1 << 31) - 1)
+        out = np.zeros(cap, dtype=np.uint8)
+        offs = np.zeros(n + 1, dtype=np.int32)
+        self._host_call(self._L.fpx_mencius_acceptor_phase1a_wire, buf.ctypes.data if len(buf) else None, len(buf),
+                        kind.ctypes.data, recs.ctypes.data, n, arena.ctypes.data if len(arena) else None,
+                        value_offsets.ctypes.data, len(value_offsets) - 1, out.ctypes.data, cap, offs.ctypes.data)
+        return out[:offs[n]].copy(), offs
+
+    def mencius_acceptor_phase1a_wire_dev(self, d_bytes, n_bytes, d_kind, d_in, n, d_arena, d_value_offsets, num_values,
+                                          d_out, out_capacity, d_offsets):
+        self._check(self._L.fpx_mencius_acceptor_phase1a_wire_dev(self.h, d_bytes, n_bytes, d_kind, d_in, n, d_arena,
+                                                                  d_value_offsets, num_values, d_out, out_capacity,
+                                                                  d_offsets))
+
+    def mencius_leader_phase1b_wire(self, leader_group, round_, chosen_watermark, buf, offsets, recover_slot=-1,
+                                    value_id_base=0, out_capacity=None):
+        """Compartmentalized Mencius' Leader.handlePhase1b of leader group leader_group over LeaderInbound bytes in
+        delivery order -> (complete, max_slot, next_slot, records P2A, spans[k, 2]): record k re-proposes slot
+        s0 + k * num_leader_groups (s0 the group's first slot >= chosen_watermark), value_id_base + k with its vote
+        value at spans[k] in buf, or VALUE_NOOP; next_slot is the leader's nextSlot afterwards.  complete = -1: no
+        quorum yet, no records.  out_capacity defaults to the engine's slot capacity."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offsets = np.ascontiguousarray(offsets, dtype=np.int32)
+        n = len(offsets) - 1
+        cap = self.cfg.slot_capacity if out_capacity is None else out_capacity
+        out = np.zeros(max(cap, 1), dtype=P2A)
+        spans = np.zeros((max(cap, 1), 2), dtype=np.int32)
+        res = np.zeros(4, dtype=np.int32)
+        self._host_call(self._L.fpx_mencius_leader_phase1b_wire, leader_group, round_, chosen_watermark, recover_slot,
+                        buf.ctypes.data if len(buf) else None, offsets.ctypes.data, n, value_id_base, out.ctypes.data,
+                        spans.ctypes.data, cap, res.ctypes.data)
+        k = int(res[2])
+        return int(res[0]), int(res[1]), int(res[3]), out[:k].copy(), spans[:k].copy()
+
+    def mencius_leader_phase1b_wire_dev(self, leader_group, round_, chosen_watermark, recover_slot, d_bytes, n_bytes,
+                                        d_offsets, n, value_id_base, d_out, d_spans, out_capacity, d_result):
+        self._check(self._L.fpx_mencius_leader_phase1b_wire_dev(self.h, leader_group, round_, chosen_watermark,
+                                                                recover_slot, d_bytes, n_bytes, d_offsets, n,
+                                                                value_id_base, d_out, d_spans, out_capacity, d_result))
+
+    def wire_encode_mencius_phase2a(self, recs, buf, spans, value_id_base=0):
+        """P2A records -> Mencius ProxyLeaderInbound{phase2a = 2} bytes, offsets[n+1], as wire_encode_phase2a
+        (mencius_leader_phase1b_wire's output as it is)."""
+        recs = np.ascontiguousarray(recs, dtype=P2A)
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        spans = np.ascontiguousarray(spans, dtype=np.int32).reshape(-1, 2)
+        k = recs["value_id"].astype(np.int64) - value_id_base
+        ok = (recs["value_id"] != VALUE_NOOP) & (k >= 0) & (k < len(spans))
+        cap = int(32 * len(recs) + spans[k[ok], 1].clip(0).sum()) + 16   # 32: the longest head
+        n = len(recs)
+        out = np.zeros(cap, dtype=np.uint8)
+        offs = np.zeros(n + 1, dtype=np.int32)
+        self._host_call(self._L.fpx_wire_encode_mencius_phase2a, recs.ctypes.data, n,
+                        buf.ctypes.data if len(buf) else None, len(buf), spans.ctypes.data, len(spans), value_id_base,
+                        out.ctypes.data, cap, offs.ctypes.data)
+        return out[:offs[n]].copy(), offs
+
+    def wire_encode_mencius_phase2a_dev(self, d_in, n, d_bytes, n_bytes, d_spans, num_spans, value_id_base, d_out,
+                                        out_capacity, d_offsets):
+        self._check(self._L.fpx_wire_encode_mencius_phase2a_dev(self.h, d_in, n, d_bytes, n_bytes, d_spans, num_spans,
+                                                                value_id_base, d_out, out_capacity, d_offsets))
+
     # -- device-pointer calls (raw device addresses, asynchronous on self.stream)
     def proxyleader_arm_dev(self, d_in, n):
         self._check(self._L.fpx_proxyleader_arm_dev(self.h, d_in, n))

@@ -1177,6 +1177,70 @@ int fpx_wire_encode_phase2a(fpx_engine* e, const fpx_p2a* in, int32_t n, const u
 int fpx_wire_encode_phase2a_dev(fpx_engine* e, const fpx_p2a* d_in, int32_t n, const uint8_t* d_bytes, int32_t n_bytes,
                                 const int32_t* d_spans, int32_t num_spans, int32_t value_id_base, uint8_t* d_out,
                                 int32_t out_capacity, int32_t* d_offsets);
+/* ---- Compartmentalized Mencius leader change from bytes (protocol FPX_MENCIUS, shard_count 1, else
+ * FPX_ERR_UNSUPPORTED; the three MultiPaxos calls above refuse FPX_MENCIUS engines).  LG = num_leader_groups, AG =
+ * num_acceptor_groups (per leader group); engine group lg * AG + ag is acceptor group ag of leader group lg.
+ *
+ * fpx_mencius_acceptor_phase1a_wire: Acceptor.handlePhase1a (S/mencius/Acceptor.scala:166-200), arguments and
+ * refusals as fpx_acceptor_phase1a_wire.  kind[] and in[] as fpx_wire_decode_inbound(FPX_WIRE_MENCIUS_ACCEPTOR_INBOUND)
+ * writes them (kind 1 = phase1a), a = engine_group << 16 | acceptor filled in by the caller.  Per acceptor, in delivery
+ * order:
+ *   1 phase1a, round < the acceptor's round -> LeaderInbound{nack = 7 {round = the acceptor's round}};
+ *   1 phase1a, otherwise                    -> round = phase1a.round and LeaderInbound{phase1b = 1 {group_index =
+ *        engine_group % AG, acceptor_index, round, info*}}: one info per voted slot >= chosen_watermark, ascending,
+ *        Phase2aNoopRange votes included (states(slot) = State(round, Noop), :263-277);
+ *   any other kind                          -> a zero-length message, nothing changed.
+ * The acceptor holds the slots s = lg + LG * ag (mod LG * AG) only; they are read from the first one >= chosen_watermark
+ * to the end of the live window (noop-range votes do not raise the max_voted_slot of fpx_snapshot_acceptor, so that
+ * cannot bound the scan). */
+int fpx_mencius_acceptor_phase1a_wire(fpx_engine* e, const uint8_t* bytes, int32_t n_bytes, const int32_t* kind,
+                                      const fpx_wire_rec* in, int32_t n, const uint8_t* arena,
+                                      const int32_t* value_offsets, int32_t num_values, uint8_t* out,
+                                      int32_t out_capacity, int32_t* offsets, int64_t* err_index);
+int fpx_mencius_acceptor_phase1a_wire_dev(fpx_engine* e, const uint8_t* d_bytes, int32_t n_bytes, const int32_t* d_kind,
+                                          const fpx_wire_rec* d_in, int32_t n, const uint8_t* d_arena,
+                                          const int32_t* d_value_offsets, int32_t num_values, uint8_t* d_out,
+                                          int32_t out_capacity, int32_t* d_offsets);
+/* fpx_mencius_leader_phase1b_wire: Leader.handlePhase1b (S/mencius/Leader.scala:582-659) of leader group
+ * leader_group, stateless like fpx_leader_phase1b_wire: the caller passes the group's round, chosenWatermark and
+ * recoverSlot (-1: the leader change was not started by a Recover; else the Recover's slot, :845-870) and the
+ * LeaderInbound bytes (Mencius.proto:322-338, nine members: a recover or chosen_watermark member after a phase1b
+ * replaces it) received since Phase 1 began.  leader_group outside [0, LG), recover_slot < -1 or chosen_watermark < 0:
+ * FPX_ERR_INVALID_ARG.  Parsing and the per-message rules as for fpx_leader_phase1b_wire, with group_index in [0, AG)
+ * (else FPX_ERR_BAD_ACCEPTOR); the quorum completes when every one of the group's AG acceptor groups holds f+1.
+ * result = {complete, max_slot, n_out, next_slot}, {-1, -1, 0, -1} while incomplete.  At completion:
+ *   max_slot  = max(maxPhase1bSlot over the held Phase1bs (-1 when empty), recover_slot); an info slot of another
+ *               leader group counts here (and fails the check below) but is never re-proposed;
+ *   max_slot != -1 and max_slot % LG != leader_group: FPX_ERR_CHECK_FAILED at complete (logger.check), nothing emitted;
+ *   s0        = nextClassicRound(leader_group, chosen_watermark - 1), the first slot >= chosen_watermark of the group;
+ *   n_out     = max_slot >= s0 ? (max_slot - s0) / LG + 1 : 0;
+ *   next_slot = nextClassicRound(leader_group, max_slot) (RoundSystem.scala:66-80), the Leader's new nextSlot (:647);
+ *               computed in 64 bits: past INT32_MAX it is FPX_ERR_SLOT_RANGE at complete (the reference's Int would
+ *               wrap; DESIGN.md §7);
+ *   record k  = {slot = s0 + k * LG, round, value_id_base + k | FPX_VALUE_NOOP, -1} with spans[2k..2k+1] as for
+ *               fpx_leader_phase1b_wire; the value is safeValue over the held Phase1bs of acceptor group (slot / LG) % AG
+ *               only (acceptorGroupIndexBySlot, :342-345), ties to the lowest acceptor index.
+ * n_out > out_capacity: FPX_ERR_INVALID_ARG at complete, nothing written.  The records go to fpx_proxyleader_arm as they
+ * are once the caller sets dst = (leader_group * AG + (slot / LG) % AG) << 16 | acceptor.  Scratch as for
+ * fpx_leader_phase1b_wire.  _dev: as fpx_leader_phase1b_wire_dev; d_result is a device int32[4]. */
+int fpx_mencius_leader_phase1b_wire(fpx_engine* e, int32_t leader_group, int32_t round, int32_t chosen_watermark,
+                                    int32_t recover_slot, const uint8_t* bytes, const int32_t* offsets, int32_t n,
+                                    int32_t value_id_base, fpx_p2a* out, int32_t* spans, int32_t out_capacity,
+                                    int32_t* result, int64_t* err_index);
+int fpx_mencius_leader_phase1b_wire_dev(fpx_engine* e, int32_t leader_group, int32_t round, int32_t chosen_watermark,
+                                        int32_t recover_slot, const uint8_t* d_bytes, int32_t n_bytes,
+                                        const int32_t* d_offsets, int32_t n, int32_t value_id_base, fpx_p2a* d_out,
+                                        int32_t* d_spans, int32_t out_capacity, int32_t* d_result);
+/* fpx_wire_encode_mencius_phase2a: Mencius' ProxyLeaderInbound{phase2a = 2 {slot, round, command_batch_or_noop}} per
+ * fpx_p2a record, otherwise as fpx_wire_encode_phase2a (the span table, FPX_VALUE_NOOP, the refusals).  Decoding the
+ * bytes with FPX_WIRE_MENCIUS_PROXYLEADER_INBOUND gives kind 2 and the records back. */
+int fpx_wire_encode_mencius_phase2a(fpx_engine* e, const fpx_p2a* in, int32_t n, const uint8_t* bytes, int32_t n_bytes,
+                                    const int32_t* spans, int32_t num_spans, int32_t value_id_base, uint8_t* out,
+                                    int32_t out_capacity, int32_t* offsets, int64_t* err_index);
+int fpx_wire_encode_mencius_phase2a_dev(fpx_engine* e, const fpx_p2a* d_in, int32_t n, const uint8_t* d_bytes,
+                                        int32_t n_bytes, const int32_t* d_spans, int32_t num_spans,
+                                        int32_t value_id_base, uint8_t* d_out, int32_t out_capacity,
+                                        int32_t* d_offsets);
 /* The replies a Client or ReadBatcher receives, by the handle's kind; out[] goes to fpx_reads_max_slot_replies[_dev]
  * as it is, spans[2i..2i+1] = {off, len} of the member's body (its last occurrence), {0, 0} for no member.
  *   FPX_READS_CLIENT, ClientInbound: max_slot_reply (4) -> {key = client_pseudonym, id = client_id,
