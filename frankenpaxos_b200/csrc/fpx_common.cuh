@@ -31,6 +31,7 @@ constexpr uint32_t kBusy = 0xfffffffdu;         // row.round_word: being moved t
 constexpr uint32_t kStampEmpty = 0xffffffffu;   // no Phase2b from this voter yet
 constexpr uint64_t kU64Empty = ~0ull;
 constexpr uint64_t kCellChosen = 0x8000000000000000ull;  // vanilla Mencius: the server's entry is a ChosenEntry
+constexpr uint64_t kCellRevocation = 0x4000000000000000ull;  // ... chosen with isRevocation (a chosen cell has no round)
 constexpr int kThreads = 256;                     // threads per CTA of the range kernels
 constexpr int kWarps = kThreads / 32;
 constexpr int kMaxKeys = FPX_MAX_ACCEPTORS;       // acceptors tracked by the round scan (lane = key)

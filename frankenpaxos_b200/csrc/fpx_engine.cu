@@ -34,6 +34,7 @@
 #include "fpx_wire.cuh"
 #include "fpx_wire_phase1.cuh"
 #include "fpx_wire_reads.cuh"
+#include "fpx_vm_revoke.cuh"
 
 using namespace fpx;
 
@@ -73,6 +74,7 @@ struct fpx_engine {
   int32_t* acc_max_voted = nullptr;
   unsigned long long* rlog = nullptr;
   uint32_t vm_tag = 1;
+  unsigned long long* vm_raise = nullptr;  // vanilla Mencius: raised entries' {voteRound, value}, on first Phase1a
   uint32_t* rng_tab = nullptr;             // mencius: (start, end, round) key table of the NoopRange path
   uint32_t* rng_tab_spare = nullptr;       // its rebuild target (fpx_retire_below)
   int32_t rng_cap = 0;
@@ -1102,7 +1104,7 @@ int fpx_vm_client_request(fpx_engine* e, const fpx_p2a* in, int32_t n, int64_t* 
                      [&](void* d) { return fpx_vm_client_request_dev(e, (const fpx_p2a*)d, n); });
 }
 
-// which: 0 handlePhase2a (d_reply dense), 1 handleChosen
+// which: 0 handlePhase2a (d_reply dense), 1 handleChosen, 2 handleChosen with isRevocation
 static int vm_launch(fpx_engine* e, const void* d_in, int32_t n, fpx_p2b* d_reply, int which) {
   int c = check_n(e, d_in, n);
   if (c != FPX_OK || n == 0) return c;
@@ -1113,7 +1115,8 @@ static int vm_launch(fpx_engine* e, const void* d_in, int32_t n, fpx_p2b* d_repl
   P.rows = e->rows; P.st = e->st;
   P.tag = e->vm_tag++;
   if (which == 0) vm_phase2a_kernel<<<std::min((n + 256 * kVmUnroll - 1) / (256 * kVmUnroll), e->num_sms * FPX_VM_CTAS_PER_SM), 256, 0, e->stream>>>(P);
-  else vm_learn_chosen_kernel<<<(n + 255) / 256, 256, 0, e->stream>>>(P);
+  else if (which == 1) vm_learn_chosen_kernel<false><<<(n + 255) / 256, 256, 0, e->stream>>>(P);
+  else vm_learn_chosen_kernel<true><<<(n + 255) / 256, 256, 0, e->stream>>>(P);
   e->launches++;
   CK(e, cudaGetLastError());
   if (e->vm_tag == 0xffffffffu) {
@@ -1151,6 +1154,12 @@ int fpx_vm_phase2a(fpx_engine* e, const fpx_p2a* in, int32_t n, fpx_p2b* reply, 
 }
 int fpx_vm_learn_chosen(fpx_engine* e, const fpx_p2b* in, int32_t n, int64_t* err_index) {
   return vm_call(e, in, n, nullptr, err_index, 1);
+}
+int fpx_vm_choose(fpx_engine* e, const fpx_p2b* in, int32_t n, int64_t* err_index) {
+  return vm_call(e, in, n, nullptr, err_index, 2);
+}
+int fpx_vm_choose_dev(fpx_engine* e, const fpx_p2b* d_in, int32_t n) {
+  return vm_launch(e, d_in, n, nullptr, 2);
 }
 
 int fpx_vm_step_dev(fpx_engine* e, const fpx_p2a* d_req, int32_t n_req, const fpx_p2a* d_p2a, int32_t n_p2a,
@@ -1310,3 +1319,4 @@ int fpx_snapshot_log(fpx_engine* e, int32_t first_slot, int32_t n_slots, int32_t
 #include "fpx_engine_reads.inc"
 #include "fpx_engine_wire_reads.inc"
 #include "fpx_engine_wire_phase1.inc"
+#include "fpx_engine_vm_revoke.inc"

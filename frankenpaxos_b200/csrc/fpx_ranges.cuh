@@ -627,6 +627,15 @@ struct VmSkipParams {
   DevStatus* st;
 };
 
+// advanceWithSkips' fill of one own slot (:613-618) at ring position l: log.put(ChosenEntry(Noop)) into a vacant
+// cell.  False where the slot is not vacant -- logger.check(!log.contains), check(!phase2s.contains) (:613-614).
+// Shared by the own = 1 skip and the self-revocation of fpx_vm_phase1a_wire.
+__device__ __forceinline__ bool vm_fill_own(const Geometry& g, unsigned long long* votes, const uint32_t* rows, int l,
+                                            int server) {
+  const unsigned long long old = atomicCAS(&votes[cell_index(g, l, server)], 0ull, kCellChosen | (uint32_t)FPX_VALUE_NOOP);
+  return old == 0ull && __ldcg(rows + (size_t)l * g.row_words) == kUnarmed;
+}
+
 __global__ void __launch_bounds__(256) vm_skip_kernel(VmSkipParams P) {
   const Geometry& g = P.g;
   const int j = blockIdx.y;
@@ -653,8 +662,7 @@ __global__ void __launch_bounds__(256) vm_skip_kernel(VmSkipParams P) {
     unsigned long long* cell = &P.votes[cell_index(g, l, server)];
     uint32_t* row = P.rows + (size_t)l * g.row_words;
     if (rec.w) {
-      unsigned long long old = atomicCAS(cell, 0ull, chosen);                      // log.put(nextSlot, ChosenEntry(Noop)) (:615-618)
-      if (old != 0ull || __ldcg(row) != kUnarmed) report_error(P.st, FPX_ERR_CHECK_FAILED, j);   // :613-614
+      if (!vm_fill_own(g, P.votes, P.rows, l, server)) report_error(P.st, FPX_ERR_CHECK_FAILED, j);
     } else {
       red_max_u64(cell, chosen);                                                      // choose: log.put (:624)
       if (slot % n == server && __ldcg(row) != kUnarmed) red_or_u32(row, kDoneBit);   // phase2s.remove(slot) (:625)

@@ -110,7 +110,8 @@ __global__ void __launch_bounds__(256, 3) vm_phase2a_kernel(VmParams P) {
       const unsigned long long mine = ((unsigned long long)(uint32_t)(rec[u].y + 1) << 32) | (uint32_t)rec[u].z;
       unsigned long long nw = old;
       if (old & kCellChosen) {
-        rk[u] = 2; rw[u] = (int)(uint32_t)old;                           // Chosen(slot, chosen.value) (:1018-1027)
+        // Chosen(slot, chosen.value, chosen.isRevocation) (:1018-1027)
+        rk[u] = (old & kCellRevocation) ? FPX_VM_REPLY_CHOSEN_REVOCATION : FPX_VM_REPLY_CHOSEN; rw[u] = (int)(uint32_t)old;
       } else if ((uint32_t)(old >> 32) > (uint32_t)(mine >> 32)) {
         rk[u] = 1; rw[u] = (int)(uint32_t)(old >> 32) - 1;               // Phase2Nack(slot, round) (:1044-1051)
       } else {
@@ -135,7 +136,10 @@ __global__ void __launch_bounds__(256, 3) vm_phase2a_kernel(VmParams P) {
   }
 }
 
-// handleChosen -> choose (:1170-1197, :622-640).  in {_, server, slot, value}
+// handleChosen -> choose (:1170-1197, :622-640).  in {is_revocation, server, slot, value}; REV = false
+// (fpx_vm_learn_chosen) does not read is_revocation.  A cell learned with and without isRevocation keeps it: the
+// cell is a max.
+template <bool REV>
 __global__ void __launch_bounds__(256) vm_learn_chosen_kernel(VmParams P) {
   const Geometry& g = P.g;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -146,7 +150,8 @@ __global__ void __launch_bounds__(256) vm_learn_chosen_kernel(VmParams P) {
   if (local < 0 && local != kLocalRetired) { report_error(P.st, FPX_ERR_SLOT_RANGE, i); return; }
   if ((uint32_t)server >= (uint32_t)g.per_group) { report_error(P.st, FPX_ERR_BAD_ACCEPTOR, i); return; }
   if (local == kLocalRetired) return;   // retired: every server's entry is a ChosenEntry already, nothing to learn
-  red_max_u64(&P.votes[cell_index(g, local, server)], kCellChosen | (uint32_t)rec.w);   // ChosenEntry (:624)
+  const unsigned long long rev = REV && rec.x != 0 ? kCellRevocation : 0ull;
+  red_max_u64(&P.votes[cell_index(g, local, server)], kCellChosen | rev | (uint32_t)rec.w);   // ChosenEntry (:624)
   if (slot % g.per_group == server) {                                                       // phase2s.remove(slot) (:625)
     uint32_t* row = P.rows + (size_t)local * g.row_words;
     if (row[0] != kUnarmed) red_or_u32(row, kDoneBit);

@@ -803,13 +803,13 @@ struct WireEncodeParams {
 
 // One message of a value-gathering encoder: outer oneof tag, int32 fields 1..nf, then (vfield != 0) the
 // value under field vfield -- arena bytes, or a vanilla Mencius Noop -- then (revocation) the required
-// `isRevocation = false` (field 3).  outer = 0: no bytes at all (a retired slot's Chosen, whose value the
+// `isRevocation` (field 3, `is_revocation`).  outer = 0: no bytes at all (a retired slot's Chosen, whose value the
 // caller holds).
 struct WireMsg {
   int outer, nf, vfield;
   int f0, f1, f2;
   int src, vlen;              // arena[src .. src + vlen); noop: CommandOrNoop{noop {}} = 12 00 instead
-  bool noop, revocation;
+  bool noop, revocation, is_revocation;
 };
 
 // value_id v of a gathering encoder; Noop (FPX_VALUE_NOOP) where the shape has one, else out of range = bad
@@ -825,7 +825,7 @@ __device__ __forceinline__ bool wire_value(const WireEncodeParams& P, int v, boo
 
 template <int KIND>
 __device__ __forceinline__ WireMsg wire_msg(const WireEncodeParams& P, int i, bool* bad) {
-  WireMsg m{0, 0, 0, 0, 0, 0, 0, 0, false, false};
+  WireMsg m{0, 0, 0, 0, 0, 0, 0, 0, false, false, false};
   if (KIND == kWireChosen) {                        // ReplicaInbound{chosen = 1 {slot = 1, command_batch_or_noop = 2}}
     const int2 r = ((const int2*)P.in)[i];
     m.outer = 0x0a; m.nf = 1; m.f0 = r.x; m.vfield = 2;
@@ -857,8 +857,10 @@ __device__ __forceinline__ WireMsg wire_msg(const WireEncodeParams& P, int i, bo
       m.outer = 0x2a; m.nf = 3; m.f0 = r.y; m.f1 = r.z; m.f2 = r.w;
     } else if (r.x == FPX_VM_REPLY_NACK) {          // phase2_nack = 9 {slot, round}
       m.outer = 0x4a; m.nf = 2; m.f0 = r.z; m.f1 = r.w;
-    } else if (r.x == FPX_VM_REPLY_CHOSEN) {        // chosen = 7 {slot, value in round, false}
+    } else if (r.x == FPX_VM_REPLY_CHOSEN || r.x == FPX_VM_REPLY_CHOSEN_REVOCATION) {
+      // chosen = 7 {slot, value in round, isRevocation}
       m.outer = 0x3a; m.nf = 1; m.f0 = r.z; m.vfield = 2; m.revocation = true;
+      m.is_revocation = r.x == FPX_VM_REPLY_CHOSEN_REVOCATION;
       *bad = !wire_value(P, r.w, true, &m);
     } else if (r.x != FPX_VM_REPLY_CHOSEN_RETIRED) {
       *bad = true;
@@ -951,7 +953,7 @@ struct WireKindCodec {
       if (m.noop) { *p++ = 0x12; *p++ = 0x00; }                // CommandOrNoop{noop = 2 {}}
       else vlen = m.vlen;
     }
-    if (m.revocation) { p[vlen] = 0x18; p[vlen + 1] = 0x00; }   // Chosen.isRevocation = 3: false
+    if (m.revocation) { p[vlen] = 0x18; p[vlen + 1] = m.is_revocation; }   // Chosen.isRevocation = 3
     *gsrc = m.src; *glen = vlen;
     return p;
   }

@@ -31,7 +31,10 @@ VM_WIRE_CLIENT_REQUEST, VM_WIRE_PHASE2A, VM_WIRE_PHASE2B, VM_WIRE_SKIP, VM_WIRE_
 
 MULTIPAXOS, MENCIUS, VANILLA_MENCIUS = 0, 1, 2
 # reply kinds of Engine.vm_phase2a (include/fpx.h FPX_VM_REPLY_*)
-VM_REPLY_PHASE2B, VM_REPLY_NACK, VM_REPLY_CHOSEN, VM_REPLY_CHOSEN_RETIRED = 0, 1, 2, 3
+VM_REPLY_PHASE2B, VM_REPLY_NACK, VM_REPLY_CHOSEN, VM_REPLY_CHOSEN_RETIRED, VM_REPLY_CHOSEN_REVOCATION = 0, 1, 2, 3, 4
+# Engine.vm_entries kinds, and the value id the engine reserves for raised entries (FPX_VALUE_RAISED)
+VM_ENTRY_NONE, VM_ENTRY_VOTELESS, VM_ENTRY_PENDING, VM_ENTRY_CHOSEN = 0, 1, 2, 3
+VALUE_RAISED = -(1 << 31) + 1
 
 OK = 0
 ERR_INVALID_ARG, ERR_CONFIG, ERR_CUDA, ERR_UNKNOWN_SLOT_ROUND, ERR_BAD_ACCEPTOR = -1, -2, -3, -4, -5
@@ -86,6 +89,36 @@ class _Handle:
         """fn(h, *args, &err_index), a host-pointer form: FpxError at the record it reports."""
         err = C.c_int64(-1)
         self._check(fn(self.h, *args, C.byref(err)), err.value)
+
+
+def _varint_fields(body):
+    """{field number: int32 value} of the varint fields of a protobuf message body (the last of each wins)."""
+    out, p = {}, 0
+    def varint():
+        nonlocal p
+        v, shift = 0, 0
+        while p < len(body):
+            c = body[p]; p += 1
+            v |= (c & 0x7f) << shift; shift += 7
+            if not c & 0x80:
+                return v
+        raise ValueError("truncated varint")
+    try:
+        while p < len(body):
+            tag = varint()
+            wt = tag & 7
+            if wt == 0:
+                v = varint() & 0xffffffff
+                out[tag >> 3] = v - (1 << 32) if v >> 31 else v
+            elif wt == 2:
+                p += varint()
+            elif wt in (1, 5):
+                p += 8 if wt == 1 else 4
+            else:
+                break
+    except ValueError:
+        pass
+    return out
 
 
 def dst(group, acceptor):
@@ -304,6 +337,57 @@ class Engine(_Handle):
         recs = np.ascontiguousarray(recs, dtype=P2B)
         self._host_call(self._L.fpx_vm_learn_chosen, recs.ctypes.data, len(recs))
 
+    def vm_choose(self, recs):
+        """Server.choose(slot, value, isRevocation) for received Chosen: {group = is_revocation, acceptor = server,
+        slot, round = value_id}."""
+        recs = np.ascontiguousarray(recs, dtype=P2B)
+        self._host_call(self._L.fpx_vm_choose, recs.ctypes.data, len(recs))
+
+    def vm_phase1a_wire(self, data, kind, recs, next_slot, arena=b"", value_offsets=(0,), out_capacity=None):
+        """Server.handlePhase1a per decoded ServerInbound record (recs.a = the receiving server).  next_slot (int32
+        per server) is updated in place.  Returns (list of reply bytes, one per record, skip records).  The default
+        out_capacity is the largest the replies can take: per Phase1a its head and one info per walked slot with the
+        arena's longest value."""
+        data = bytes(data)
+        kind = np.ascontiguousarray(kind, dtype=np.int32)
+        recs = np.ascontiguousarray(recs, dtype=WIRE_REC)
+        vo = np.ascontiguousarray(value_offsets, dtype=np.int32)
+        n = len(kind)
+        if out_capacity is None:
+            vmax = max([2] + [int(x) for x in np.diff(vo)])
+            out_capacity = 64
+            for i in np.nonzero(kind == 2)[0]:
+                r = recs[i]
+                f = _varint_fields(data[max(int(r["c"]), 0): max(int(r["c"]), 0) + max(int(r["d"]), 0)])
+                start, stop, servers = f.get(2, 0), f.get(3, 0), self.cfg.acceptors_per_group
+                walked = (stop - start + servers - 1) // servers if 0 <= start < stop else 0
+                out_capacity += 64 + walked * (48 + vmax)
+        out = np.empty(max(out_capacity, 1), dtype=np.uint8)
+        offs = np.zeros(n + 1, dtype=np.int32)
+        skips = np.zeros(max(n, 1), dtype=VM_SKIP)
+        a = np.frombuffer(bytes(arena) + b"\0", dtype=np.uint8)
+        b = np.frombuffer(data + b"\0", dtype=np.uint8)
+        assert next_slot.dtype == np.int32 and next_slot.flags.c_contiguous
+        self._host_call(self._L.fpx_vm_phase1a_wire, b.ctypes.data, len(data), kind.ctypes.data, recs.ctypes.data, n,
+                        a.ctypes.data, vo.ctypes.data, len(vo) - 1, next_slot.ctypes.data, out.ctypes.data,
+                        out_capacity, offs.ctypes.data, skips.ctypes.data)
+        return [out[offs[i]:offs[i + 1]].tobytes() for i in range(n)], skips[:n]
+
+    def vm_phase1a_wire_dev(self, d_bytes, n_bytes, d_kind, d_in, n, d_arena, d_value_offsets, num_values, d_next_slot,
+                            d_out, out_capacity, d_offsets, d_skips):
+        self._check(self._L.fpx_vm_phase1a_wire_dev(self.h, d_bytes, n_bytes, d_kind, d_in, n, d_arena, d_value_offsets,
+                                                    num_values, d_next_slot, d_out, out_capacity, d_offsets, d_skips))
+
+    def vm_choose_dev(self, d_in, n):
+        self._check(self._L.fpx_vm_choose_dev(self.h, d_in, n))
+
+    def vm_entries(self, server, first_slot, n_slots):
+        """server's entries at [first_slot, first_slot + n_slots): int32 [n_slots, 5] {kind (VM_ENTRY_*), round,
+        voteRound, value, isRevocation}."""
+        out = np.zeros((max(n_slots, 1), 5), dtype=np.int32)
+        self._check(self._L.fpx_vm_entries(self.h, server, first_slot, n_slots, out.ctypes.data))
+        return out[:n_slots]
+
     def vm_skip(self, recs):
         """Server.advanceWithSkips' log fill (own=1) / Server.handleSkip (own=0)."""
         recs = np.ascontiguousarray(recs, dtype=VM_SKIP)
@@ -462,7 +546,7 @@ class Engine(_Handle):
         """The dense reply stream of vm_phase2a / vm_step_dev -> (bytes, offsets[n+1]); a kind-3 reply
         (VM_REPLY_CHOSEN_RETIRED) is a zero-length message: the caller holds that slot's value."""
         replies = np.ascontiguousarray(replies, dtype=P2B)
-        vids = np.where(replies["group"] == VM_REPLY_CHOSEN, replies["round"], -1)
+        vids = np.where(np.isin(replies["group"], (VM_REPLY_CHOSEN, VM_REPLY_CHOSEN_REVOCATION)), replies["round"], -1)
         return self._wire_encode_valued(self._L.fpx_wire_encode_vm_replies, replies, P2B, vids, arena, value_offsets)
 
     def wire_encode_vm_chosen(self, recs, arena=None, value_offsets=None):

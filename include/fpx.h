@@ -281,8 +281,8 @@ int fpx_leader_safe_values(fpx_engine* e, uint32_t responders, int32_t first_slo
  * n = 2f+1 servers (acceptors_per_group = n, num_acceptor_groups = 1), every
  * server is proposer + acceptor, server s coordinates the slots with slot % n ==
  * s.  One engine holds the log entries of all n servers (vote cells [slot][server])
- * and the coordinators' `phase2s`.  Skips, revocation and Phase 1 are control
- * path and out of scope (SURVEY.md 8(a) row a9).  Batch contract (checked, ->
+ * and the coordinators' `phase2s`.  Skips are below; the servers' side of a
+ * revocation's Phase 1 is the block after them.  Batch contract (checked, ->
  * FPX_ERR_BATCH_ORDER): at most one Phase2a per (slot, server) per call, because
  * the round compare is per log entry (:1016-1042), not per acceptor.  The key is
  * in the message, so a caller can always flush ahead of a repeat; a call that
@@ -290,7 +290,9 @@ int fpx_leader_safe_values(fpx_engine* e, uint32_t responders, int32_t first_slo
 
 /* Server.handleClientRequest, state part (:767-829): the coordinator in.dst (which
  * must own in.slot) votes for its own command -- log(slot) = PendingEntry(0, 0,
- * value) (:779) -- and opens phase2s(slot) with its own Phase2b (:818-825). */
+ * value) (:779) -- and opens phase2s(slot) with its own Phase2b (:818-825).
+ * Value ids here and in fpx_vm_phase2a must not be FPX_VALUE_RAISED (INT32_MIN + 1), which marks
+ * an entry raised by a revocation's Phase1a (fpx_vm_phase1a_wire); the hot path does not check it. */
 int fpx_vm_client_request(fpx_engine* e, const fpx_p2a* in, int32_t n, int64_t* err_index);
 
 /* Server.handlePhase2a (:1001-1082) at server in.dst.  DENSE replies, reply[i]
@@ -302,8 +304,11 @@ int fpx_vm_client_request(fpx_engine* e, const fpx_p2a* in, int32_t n, int64_t* 
  *           Chosen(slot, value) (:1016-1025), but the engine no longer holds the value: it is the
  *           shared log's executed entry of the slot, which the caller holds.  This is the one reply
  *           that differs from the reference's; a server that had not learned the slot before it was
- *           retired would have answered Phase2b or Phase2Nack there, and gets kind 3 here as well. */
-enum { FPX_VM_REPLY_PHASE2B = 0, FPX_VM_REPLY_NACK = 1, FPX_VM_REPLY_CHOSEN = 2, FPX_VM_REPLY_CHOSEN_RETIRED = 3 };
+ *           retired would have answered Phase2b or Phase2Nack there, and gets kind 3 here as well.
+ *   kind 4  Chosen(slot, value in `round`, isRevocation = true): the entry was chosen by a revocation
+ *           (fpx_vm_choose with is_revocation = 1).  Without revocation, kind 4 never occurs. */
+enum { FPX_VM_REPLY_PHASE2B = 0, FPX_VM_REPLY_NACK = 1, FPX_VM_REPLY_CHOSEN = 2, FPX_VM_REPLY_CHOSEN_RETIRED = 3,
+       FPX_VM_REPLY_CHOSEN_REVOCATION = 4 };
 int fpx_vm_phase2a(fpx_engine* e, const fpx_p2a* in, int32_t n, fpx_p2b* reply, int64_t* err_index);
 /* device-pointer forms (asynchronous on the engine's stream, errors surface at fpx_sync) */
 int fpx_vm_client_request_dev(fpx_engine* e, const fpx_p2a* d_in, int32_t n);
@@ -327,6 +332,29 @@ int fpx_vm_learn_chosen(fpx_engine* e, const fpx_p2b* in, int32_t n, int64_t* er
  * handleSkip (:1144-1168) at `server`: choose(slot, Noop) for the coordinator's slots of
  * the range (log.put unconditionally, phase2s.remove, :622-625).  n <= FPX_MAX_RANGE_BATCH. */
 int fpx_vm_skip(fpx_engine* e, const fpx_vm_skip_rec* in, int32_t n, int64_t* err_index);
+
+/* ---- Vanilla Mencius revocation, the servers' side (protocol FPX_VANILLA_MENCIUS, shard_count 1; any other:
+ * FPX_ERR_UNSUPPORTED) ----
+ * Revocation keeps Mencius live after a server fails: another server (the revoker, round % n of a round >= n)
+ * runs Phase 1 over the failed server's slots [start, stop) and fills them in.  Besides PendingEntry and
+ * ChosenEntry an entry can now be VotelessEntry(round) or a PendingEntry whose round was raised above its
+ * voteRound, and a ChosenEntry carries isRevocation.  FPX_VALUE_RAISED is a value id the engine reserves for
+ * raised entries: a Phase2a must not carry it.  The revoker's fill-in and its Phase 2 are the caller's. */
+#define FPX_VALUE_RAISED (INT32_MIN + 1)
+
+/* Server.handleChosen -> choose(slot, value, isRevocation) (:1170-1197, :622-640) at server in.acceptor.  Record
+ * fields: group = is_revocation (nonzero: true), acceptor = the learning server, slot, round = the value id.  A
+ * decoder kind-7 row {slot, is_revocation, value_off, value_len} becomes {b, server, a, the caller's value id for
+ * the span}.  fpx_vm_learn_chosen is this call with is_revocation = 0 (it does not read group).  A ChosenEntry learned both with and without
+ * isRevocation keeps isRevocation = true (the reference keeps the last delivered; the value is the same). */
+int fpx_vm_choose(fpx_engine* e, const fpx_p2b* in, int32_t n, int64_t* err_index);
+int fpx_vm_choose_dev(fpx_engine* e, const fpx_p2b* d_in, int32_t n);
+
+/* Read-only snapshot of server `server`'s entries at slots [first_slot, first_slot + n_slots), all live
+ * (FPX_ERR_SLOT_RANGE otherwise): out[5 * k ..] = {kind (0 none, 1 VotelessEntry, 2 PendingEntry, 3 ChosenEntry),
+ * round, voteRound (-1 for none and Voteless), value (Pending and Chosen), isRevocation (Chosen)}; 0 where a
+ * kind has no such field. */
+int fpx_vm_entries(fpx_engine* e, int32_t server, int32_t first_slot, int32_t n_slots, int32_t* out);
 
 /* ---- Mencius Phase2aNoopRange path (S/mencius), protocol FPX_MENCIUS ---------------
  * A lagging leader group closes its gap with ONE message standing for the strided run
@@ -484,11 +512,12 @@ int fpx_wire_decode_vm_server_inbound_dev(fpx_engine* e, const uint8_t* d_bytes,
                                           int32_t* d_kind, fpx_wire_rec* d_out, int32_t* d_sender);
 /* Encoders: canonical ServerInbound bytes, one message per record.  Values: value_id v is the CommandOrNoop
  * arena[value_offsets[v] .. value_offsets[v+1]); FPX_VALUE_NOOP is CommandOrNoop{noop {}} (bytes 12 00); any
- * other value_id outside [0, num_values) is FPX_ERR_INVALID_ARG at that record.  isRevocation is always written
- * false (18 00): the engine has no revocation.
+ * other value_id outside [0, num_values) is FPX_ERR_INVALID_ARG at that record.  isRevocation is written false
+ * (18 00) except for reply kind 4.
  * _vm_replies: the dense reply stream of fpx_vm_phase2a[_dev] / fpx_vm_step_dev, by reply kind:
  *   0 phase2b{server_index = acceptor, slot, round}   1 phase2_nack{slot, round}
  *   2 chosen{slot, command_or_noop = the value in `round`, false}
+ *   4 (FPX_VM_REPLY_CHOSEN_REVOCATION) chosen{slot, the value in `round`, true}
  *   3 (FPX_VM_REPLY_CHOSEN_RETIRED) a ZERO-LENGTH message: the engine no longer holds the retired slot's value;
  *     the caller, which holds the executed entry, sends that Chosen itself.
  *   Any other kind is FPX_ERR_INVALID_ARG at that record. */
@@ -518,6 +547,36 @@ int fpx_wire_encode_vm_skip(fpx_engine* e, const fpx_vm_skip_rec* in, int32_t n,
                             int32_t* offsets, int64_t* err_index);
 int fpx_wire_encode_vm_skip_dev(fpx_engine* e, const fpx_vm_skip_rec* d_in, int32_t n, uint8_t* d_out,
                                 int32_t out_capacity, int32_t* d_offsets);
+
+/* The servers' side of a revocation (see fpx_vm_choose above). */
+/* Server.handlePhase1a (:831-911) from bytes.  kind[] / in[] are fpx_wire_decode_vm_server_inbound's rows of the
+ * ServerInbound batch `bytes` (kind 2: {0, 0, body_off, body_len}) with in[i].a set by the caller to the receiving
+ * server.  Values: the caller's CommandOrNoop arena as for the encoders above.  next_slot[n] (in / out) holds
+ * every server's nextSlot, as for fpx_vm_skip.  Per server, in delivery order, each Phase1a{round, start, stop}:
+ *   - if start mod n is the receiving server, the log fill of advanceWithSkips(stop - 1) first (as an own = 1
+ *     fpx_vm_skip, FPX_ERR_CHECK_FAILED where a slot is not vacant); skips[i] = {server, old next_slot, new stop,
+ *     1}, the range for the caller's skipSlots (slot_start == slot_stop: none), and next_slot advances;
+ *   - the walk over start, start + n, ... < stop: no entry becomes VotelessEntry(round); a Voteless or Pending
+ *     entry above the round stops the walk with ServerInbound{phase1_nack = 8 {start, stop, entry's round}} -- the
+ *     entries before it stay raised; a PendingEntry adds PendingSlotInfo{voteRound, voteValue} and takes the round;
+ *     a ChosenEntry adds ChosenSlotInfo{value, isRevocation};
+ *   - otherwise the reply is ServerInbound{phase1b = 3 {server_index, round, start, stop, info...}}.
+ * out / offsets[n + 1]: one reply per record, zero-length for any other kind.  Refused with nothing applied:
+ * malformed bytes or a missing field (FPX_ERR_WIRE), a server out of range or a next_slot not of its server
+ * (FPX_ERR_INVALID_ARG), a round outside [0, FPX_MAX_ROUND] (FPX_ERR_ROUND_RANGE), start < 0, a walked slot or a
+ * slot of the fill that is retired or beyond the live window, or a next_slot past INT32_MAX (FPX_ERR_SLOT_RANGE;
+ * the caller sizes slot_capacity to cover nextSlot + 2 beta).  Found only after the entries are raised (fatal,
+ * like every half-applied call): a value id outside the arena in a reply (FPX_ERR_INVALID_ARG at that record) and
+ * replies longer than out_capacity (FPX_ERR_INVALID_ARG at 0). */
+int fpx_vm_phase1a_wire(fpx_engine* e, const uint8_t* bytes, int32_t n_bytes, const int32_t* kind,
+                        const fpx_wire_rec* in, int32_t n, const uint8_t* arena, const int32_t* value_offsets,
+                        int32_t num_values, int32_t* next_slot, uint8_t* out, int32_t out_capacity, int32_t* offsets,
+                        fpx_vm_skip_rec* skips, int64_t* err_index);
+/* device-pointer form: d_out, d_in and d_skips 16-byte aligned; synchronises once to size its scratch */
+int fpx_vm_phase1a_wire_dev(fpx_engine* e, const uint8_t* d_bytes, int32_t n_bytes, const int32_t* d_kind,
+                            const fpx_wire_rec* d_in, int32_t n, const uint8_t* d_arena, const int32_t* d_value_offsets,
+                            int32_t num_values, int32_t* d_next_slot, uint8_t* d_out, int32_t out_capacity,
+                            int32_t* d_offsets, fpx_vm_skip_rec* d_skips);
 
 /* ---- Wire codec of Compartmentalized Mencius' noop ranges and replica (protocol FPX_MENCIUS; any other:
  * FPX_ERR_UNSUPPORTED) ----
